@@ -1,11 +1,11 @@
 #!/usr/bin/env python
 """Headline benchmark: data-parallel ResNet-50 (bf16) synthetic training throughput.
 
-This is the reference's own benchmark (/root/reference/example/pytorch/benchmark_byteps.py:
+This is the reference's own benchmark (example/pytorch/benchmark_byteps.py of bytedance/byteps:
 torchvision-style ResNet-50, synthetic 3x224x224 batches, SGD lr=0.01 wrapped in
 ``DistributedOptimizer``, img/sec = batch * steps / time, total = per-GPU * size),
 run through OUR public API, in the configuration BASELINE.json names
-("ResNet-50 data-parallel bf16 on 8xB200"; batch 64 per GPU as in the
+("ResNet-50 data-parallel bf16 on 8xH100"; batch 64 per GPU as in the
 reference's published ResNet-50 numbers, docs/performance.md).
 
     python bench.py --gpus 1 --steps 50 --warmup 10
@@ -21,6 +21,10 @@ path (per-partition reduce-scatter/all-gather + div, unfused optimizer) and
 `--impl ddp` the strongest library baseline on the same box (torch DDP, NCCL
 bucketed all-reduce, fused torch optimizer, whole step captured in the same
 CUDA graph) for our own comparison tables.
+
+`--dump-outputs DIR` writes, on rank 0, what the last device-timed step computed: its loss and a fixed,
+seeded sample of the updated parameters, as float32 .npy files.  Model weights and batches are seeded, so
+two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -52,16 +56,32 @@ def parse():
     ap.add_argument("--no-graph", action="store_true", help="disable whole-step CUDA graph capture")
     ap.add_argument("--no-fused", action="store_true", help="unfused optimizer (gradient all-gather + torch step)")
     ap.add_argument("--no-e2e", action="store_true")
-    ap.add_argument("--cudnn-benchmark", action="store_true",
-                    help="cuDNN autotuning: measured no faster than the heuristics on B200 (14.2 vs 14.1 ms/step) "
-                         "and 25-45 s slower to start")
+    ap.add_argument("--cudnn-benchmark", action="store_true", help="cuDNN autotuning (slower to start)")
     ap.add_argument("--verbose", action="store_true", help="phase progress on stderr (all ranks)")
     ap.add_argument("--hang-dump", type=float, default=float(os.environ.get("BENCH_HANG_DUMP_S", "0")),
                     help="dump python stacks of every thread to stderr every N seconds (debugging hangs)")
     ap.add_argument("--momentum", type=float, default=0.0)
     ap.add_argument("--optimizer", default="auto", choices=["auto", "sgd", "adamw"],
                     help="auto: SGD lr=0.01 for CNNs (the reference benchmark), AdamW for BERT")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the loss and a seeded sample of the parameters after the last timed step as .npy")
     return ap.parse_args()
+
+
+DUMP_PARAM_SAMPLE = 1 << 22     # 4 Mi float32 parameters (16 MB), well under the 64 MB the dump may take
+
+
+def dump_outputs(out_dir, torch, model, loss):
+    """loss.npy: the last timed step's loss; params_sample.npy: DUMP_PARAM_SAMPLE entries of all parameters after
+    that step's update, flattened in model.parameters() order, at sorted indices drawn with a fixed seed."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    flat = torch.cat([p.detach().float().reshape(-1) for p in model.parameters()])
+    idx = torch.from_numpy(np.sort(np.random.default_rng(0).choice(flat.numel(), min(DUMP_PARAM_SAMPLE, flat.numel()),
+                                                                   replace=False)))
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().float().reshape(1).cpu().numpy())
+    np.save(os.path.join(out_dir, "params_sample.npy"), flat[idx.to(flat.device)].cpu().numpy())
 
 
 class ClockSampler:
@@ -229,6 +249,7 @@ def main():
         bps = _TorchDist(torch, world, local_rank)      # noqa: F811 - the baseline arm must not touch our engine
     bps.init()
     note("init done")
+    torch.manual_seed(0)                            # same initial weights on every run (rank 0's are broadcast)
     model, host, sx, sy, is_bert = build(args, torch, bps, device)
     note("model built")
     fused = not args.no_fused and args.impl == "ours"
@@ -326,7 +347,10 @@ def main():
     if bps.rank() == 0:
         sampler.start()
     # ---- device-timed region: inputs resident on the device (the reference's benchmark does the same)
-    ms = timed(lambda i: stepper(), args.steps)
+    last = [None]
+    ms = timed(lambda i: last.__setitem__(0, stepper()), args.steps)
+    if args.dump_outputs and bps.rank() == 0:
+        dump_outputs(args.dump_outputs, torch, model, last[0])
     note("device-timed region done: %.3f ms/step" % (ms / args.steps))
     if use_graph:
         # kernels of ours inside one captured step (graph replays do not pass through python launch counters)
@@ -423,7 +447,7 @@ def main():
                                      else "SGD lr=0.01 momentum=%g" % args.momentum),
                        "fused_update": fused, "cuda_graph": use_graph, "params": nparams,
                        "l2": "no explicit flush: a step streams weights+activations+gradients far larger than "
-                             "the 126 MB L2",
+                             "the 50 MB L2 of an H100",
                        "backend": eng.backend if eng is not None else "torch DDP + NCCL",
                        "ring": getattr(getattr(opt, "grad_sync", None), "_ring_mode", None),
                        "graph_note": graph_note},

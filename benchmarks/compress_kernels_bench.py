@@ -50,7 +50,7 @@ def main():
         comp = GpuCompressor(_Ctx(vc, 0), kw, n, torch.float32)
         tot = None
         for it in range(args.iters + 2):
-            flush.fill_(it & 1)                       # evict the 126 MB L2 between iterations
+            flush.fill_(it & 1)                       # evict the 50 MB L2 between iterations
             phases = comp.phases(g, out, True, s.cuda_stream)
             evs = [torch.cuda.Event(enable_timing=True) for _ in range(len(phases) + 1)]
             evs[0].record()

@@ -70,7 +70,8 @@ def main():
 
     blob = struct.pack("<9f3if3i", 0.01, 1e-4, 0.9, 0.0, 0.9, 0.999, 1e-8, 0.1, 0.001, 0, 0, 0, 1.0, 0, 0, 0)
     cu.write_blob(hp.data_ptr(), blob, s)
-    blocks = 148 * 2
+    sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+    blocks = sms * 2
     # fused SGD+momentum: read g(2) + w(4) + m(4), write w(4) + m(4) + p(2) = 20 B/elem
     timed(lambda: cu.pushpull_fused_opt(view, 1, 1, 1, cu.OPT_SGD, 0, 0, goff, poff, n, 1.0, master.data_ptr(),
                                         mom.data_ptr(), 0, hp.data_ptr(), blocks, 512, 0, False, s),
@@ -81,16 +82,16 @@ def main():
           n * 28, "fused_opt_adam_bf16")
     # same two optimizers with the state streamed through shared memory by bulk copies (TMA variant)
     timed(lambda: cu.pushpull_fused_opt_tma(view, 1, cu.OPT_SGD, goff, poff, n, 1.0, master.data_ptr(), mom.data_ptr(),
-                                            0, hp.data_ptr(), 296, 6, False, 0, s),
+                                            0, hp.data_ptr(), blocks, 6, False, 0, s),
           n * 20, "fused_opt_tma_sgd_momentum_bf16")
     timed(lambda: cu.pushpull_fused_opt_tma(view, 1, cu.OPT_ADAM, goff, poff, n, 1.0, master.data_ptr(),
-                                            mom.data_ptr(), m2.data_ptr(), hp.data_ptr(), 296, 4, False, 0, s),
+                                            mom.data_ptr(), m2.data_ptr(), hp.data_ptr(), blocks, 4, False, 0, s),
           n * 28, "fused_opt_tma_adam_bf16")
     for nb in [int(x) for x in args.sweep_blocks.split(",") if x]:
         timed(lambda: cu.pushpull_fused_opt_tma(view, 1, cu.OPT_ADAM, goff, poff, n, 1.0, master.data_ptr(),
                                                 mom.data_ptr(), m2.data_ptr(), hp.data_ptr(), nb, 4, False, 0, s),
               n * 28, "fused_opt_tma_adam_bf16[blocks=%d,stages=4]" % nb)
-        if nb <= 148:
+        if nb <= sms:
             timed(lambda: cu.pushpull_fused_opt_tma(view, 1, cu.OPT_ADAM, goff, poff, n, 1.0, master.data_ptr(),
                                                     mom.data_ptr(), m2.data_ptr(), hp.data_ptr(), nb, 8, False, 0, s),
                   n * 28, "fused_opt_tma_adam_bf16[blocks=%d,stages=8]" % nb)

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Summarise an .ncu-rep (read on the CPU box with `ncu -i`) into profiles/<name>.md.
 
-    python benchmarks/ncu_summary.py gpurun_out/prof_fused_opt.ncu-rep profiles/ncu_fused_opt.md
+    python benchmarks/ncu_summary.py <report>.ncu-rep <summary>.md
 """
 import csv
 import io
@@ -24,7 +24,7 @@ def main():
     rows = list(csv.reader(io.StringIO(raw)))
     hdr, units, data = rows[0], rows[1], rows[2:]
     with open(out, "w") as f:
-        f.write("# ncu summary of %s\n\n`ncu --set full --clock-control none --import-source on` on one B200; "
+        f.write("# ncu summary of %s\n\n`ncu --set full --clock-control none --import-source on` on one H100; "
                 "read here with `ncu -i ... --page raw --csv`.\n\n" % rep)
         for r in data:
             d = dict(zip(hdr, r))

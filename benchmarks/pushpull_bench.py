@@ -12,7 +12,7 @@ events and max over ranks:
 
 bus GB/s = 2*(N-1)/N * bytes / time, the NCCL-tests convention.  Roofline: the
 P2P kernel moves 2*(N-1)/N*S bytes per GPU per direction -> bus GB/s is bounded
-by the per-direction NVLink bandwidth (measured peer copy: 770 GB/s).
+by the per-direction NVLink bandwidth (H100, NVLink 4: 450 GB/s nominal).
 """
 import argparse
 import json
@@ -55,7 +55,7 @@ def main():
     ap.add_argument("--out", default="")
     ap.add_argument("--sizes", default="65536,1048576,4194304,16777216,104857600,536870912")
     ap.add_argument("--quick", action="store_true",
-                    help="bf16 only, one grid per variant, no TMA/tcgen05/reference-style sweeps (short GPU leases)")
+                    help="bf16 only, one grid per variant, no TMA/wgmma/reference-style sweeps (short GPU leases)")
     ap.add_argument("--skip-api", action="store_true", help="skip the per-tensor public-API gradient sets")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", 0))
@@ -78,7 +78,7 @@ def main():
                       "try" if eng.cfg.use_nvls == "auto" else eng.cfg.use_nvls)   # measure NVLS at any world size
     stream = torch.cuda.current_stream(device)
     ref = NcclReferencePath()
-    # L2 flush buffer (> 126 MB)
+    # L2 flush buffer (> the 50 MB L2)
     fl = torch.empty(256 << 20, dtype=torch.uint8, device=device)
 
     def flush():
@@ -123,7 +123,7 @@ def main():
             if dt == torch.bfloat16 and world <= 8 and not args.quick:
                 maps = cu.make_umma_maps(ctx.view, wire_code(dt), 0, n)
                 best = None
-                for cap in (8, 16, 32, 64, 148):
+                for cap in (8, 16, 32, 64, torch.cuda.get_device_properties(device).multi_processor_count):
                     blocks = max(1, min(cap, (shard + 16383) // 16384))
                     if best is not None and blocks == best[1]:
                         continue
@@ -132,7 +132,7 @@ def main():
                                args.iters, args.warmup, device, flush)
                     if best is None or ms < best[0]:
                         best = (ms, blocks)
-                rows.append({"what": "ours_inplace_tcgen05_tma", "bytes": nbytes, "dtype": str(dt)[6:], "ms": best[0],
+                rows.append({"what": "ours_inplace_wgmma_tma", "bytes": nbytes, "dtype": str(dt)[6:], "ms": best[0],
                              "blocks": best[1], "alg_gbs": nbytes / best[0] / 1e6,
                              "bus_gbs": factor * nbytes / best[0] / 1e6})
             y = torch.ones(n, dtype=dt, device=device)

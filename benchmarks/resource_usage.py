@@ -43,7 +43,7 @@ def main():
         t["local"] = max(t["local"], loc)
         if tmpl:
             t["variants"].append((tmpl.group(1).replace("bps::", ""), reg))
-    print("# Static resource usage of the sm_100a kernels\n")
+    print("# Static resource usage of the sm_90a kernels\n")
     print("`python benchmarks/resource_usage.py` (cuobjdump --dump-resource-usage on the in-tree `_cuda` module; no GPU "
           "needed).  %d kernel instantiations of %d kernels.  `stack`/`local` > 0 would mean spills or dynamically "
           "indexed arrays in a hot loop; the 16 B (32 B) stack of the cross-rank kernels is the argument block of the barrier "
@@ -55,8 +55,8 @@ def main():
         print("| `%s` | %d | %d-%d | %d | %d | %d |" % (k, t["n"], min(t["reg"]), max(t["reg"]), t["stack"], t["shared"],
                                                        t["local"]))
     print("\nDynamic shared memory (not in the table): TMA push-pull ring `stages x (world+1) x 4 KiB`, fused-optimizer "
-          "ring `stages x streams x 256 x 16|32 B` (<= 96 KiB so that two CTAs share an SM), tcgen05 variant "
-          "`stages x (P x 16 KiB B tiles) + A`.")
+          "ring `stages x streams x 256 x 16|32 B` (<= 96 KiB so that two CTAs share an SM), wgmma variant "
+          "`6 x 16 KiB peer tiles + a 16 KiB output tile`.")
 
 
 if __name__ == "__main__":

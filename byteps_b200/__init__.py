@@ -1,4 +1,4 @@
-"""byteps_b200 - a Blackwell-native gradient synchronisation engine with the
+"""byteps_b200 - a Hopper-native gradient synchronisation engine with the
 capabilities and Horovod-style API of bytedance/byteps.
 
 Layer map (see SURVEY.md section 1 for the reference's):
@@ -7,7 +7,7 @@ Layer map (see SURVEY.md section 1 for the reference's):
 * ``byteps_b200.common``    - process-wide state: ranks, config, engine lifecycle
 * ``byteps_b200.comm``      - transports: symmetric-memory CUDA kernels, NCCL
                               baseline, gloo plumbing, parameter-server client
-* ``byteps_b200.ops``       - python wrappers of the sm_100a kernels
+* ``byteps_b200.ops``       - python wrappers of the sm_90a kernels
 * ``byteps_b200.parallel``  - DistributedDataParallel, CrossBarrier, sharded fused optimizers
 * ``byteps_b200.models``    - benchmark model zoo (ResNet/VGG/BERT/MNIST)
 * ``byteps_b200.server``    - the CPU summation server (``import byteps_b200.server`` runs it)

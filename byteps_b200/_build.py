@@ -4,9 +4,9 @@ Two extension modules are produced next to this file:
 
 * ``_core``  - pure C++17 runtime (registry, scheduler, CPU reducer, compressors,
   KV transport, server).  No CUDA, no torch headers: builds and runs on a CPU box.
-* ``_cuda``  - sm_100a CUDA kernels (fused push-pull over NVLink peer memory,
+* ``_cuda``  - sm_90a CUDA kernels (fused push-pull over NVLink peer memory,
   compression, fused optimizers) + symmetric-memory setup.  Cross-compiled with
-  ``nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo``.
+  ``nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo``.
 
 The reference builds everything through one ``setup.py`` with host-only flags
 (/root/reference/setup.py:177-230); we keep builds incremental and in-tree so
@@ -28,7 +28,7 @@ CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "build")
 EXT = sysconfig.get_config_var("EXT_SUFFIX")
 
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def _py_includes():
@@ -120,7 +120,7 @@ def _save_stamps(s):
 import platform
 
 _X86 = platform.machine().lower() in ("x86_64", "amd64", "i386", "i686")
-# BYTEPS_NO_X86_SIMD=1: build the scalar fallbacks only (what an aarch64 host - e.g. a Grace-based Blackwell system -
+# BYTEPS_NO_X86_SIMD=1: build the scalar fallbacks only (what an aarch64 host - e.g. a Grace Hopper system -
 # gets automatically); used by the tests to check that the fallbacks are complete
 _SIMD = _X86 and os.environ.get("BYTEPS_NO_X86_SIMD", "0") in ("0", "")
 CXX_FLAGS = [
@@ -171,7 +171,7 @@ NVCC_FLAGS = [
 def build_cuda(verbose=False, force=False, ptxas_verbose=False):
     nvcc = _nvcc()
     if nvcc is None:
-        raise RuntimeError("nvcc not found; cannot build the sm_100a extension")
+        raise RuntimeError("nvcc not found; cannot build the sm_90a extension")
     os.makedirs(BUILD, exist_ok=True)
     stamps = _load_stamps()
     hs = _headers_stamp()

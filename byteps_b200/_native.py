@@ -33,7 +33,7 @@ def core():
 
 
 def cuda():
-    """The sm_100a extension.  Fails loudly if it cannot be built/loaded: a GPU
+    """The sm_90a extension.  Fails loudly if it cannot be built/loaded: a GPU
     box must never silently fall back to eager PyTorch."""
     global _cuda
     if _cuda is None:

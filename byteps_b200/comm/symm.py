@@ -4,7 +4,7 @@ A :class:`SymmContext` is one peer-mapped device allocation (data window +
 signal pad) shared by all ranks of a job, plus the ``PeerView`` the kernels
 take.  Creation is collective.  :class:`VirtualCluster` builds N "virtual
 ranks" inside ONE process on ONE GPU, which lets the multi-peer kernels be
-tested for numerics on a single B200 (the N kernels run concurrently on N
+tested for numerics on a single H100 (the N kernels run concurrently on N
 streams and synchronise through the same flag protocol).
 """
 from __future__ import annotations
@@ -70,8 +70,8 @@ class SymmContext:
             stamp("symm: peers imported")
             group.barrier()
         self.nvls = False
-        # auto: in-switch reduction pays from 4 peers up (8 GPUs: 734 vs 581 GB/s bus at 100 MB); with
-        # 2 peers plain P2P loads are faster (538 vs 364 GB/s) - see profiles/pushpull_nvlink.md
+        # auto: in-switch reduction from 4 peers up; with 2 peers plain P2P loads (fewer multimem protocol bytes
+        # per useful byte)
         want_nvls = use_nvls in ("1", "try") or (use_nvls == "auto" and self.world >= 4)
         if self.world > 1 and want_nvls and self.mem.mode == "vmm":
             self._setup_multicast(required=(use_nvls == "1"))
@@ -152,9 +152,9 @@ class VirtualCluster:
             cur.wait_stream(s)
 
 
-def pick_blocks(shard_bytes: int, threads: int, unroll_bytes: int, cap: int, sm_count: int = 148) -> int:
+def pick_blocks(shard_bytes: int, threads: int, unroll_bytes: int, cap: int, sm_count: int = 132) -> int:
     """CTAs for an exchange: enough tiles in flight to cover the NVLink
-    bandwidth-delay product (~2 us x 770 GB/s = 1.5 MB per GPU) without
+    bandwidth-delay product (~2 us x 450 GB/s of NVLink 4 = 0.9 MB per GPU) without
     taking every SM away from the backward pass."""
     tile = threads * unroll_bytes
     need = max(1, (shard_bytes + tile - 1) // tile)

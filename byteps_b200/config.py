@@ -55,7 +55,7 @@ class Config:
     omp_threads: int = 4
     threadpool_size: int = 4
     server_engine_threads: int = 4
-    # ---- B200 data path
+    # ---- H100 data path
     backend: str = "auto"                # auto | symm | nccl | gloo | ps | local
     symm_mode: str = "auto"              # auto | vmm | ipc
     arena_bytes: int = 256 << 20

@@ -281,8 +281,8 @@ PYBIND11_MODULE(_core, m) {
           "fill_randint_u32",
           [](XorShift128Plus& r, uintptr_t ptr, size_t k, uint64_t high) {
             // k draws of randint(0, high) into a host buffer (random-k index streams for the GPU
-            // compressor: the generator is inherently serial, 250 k draws cost < 1 ms here and
-            // 90 ms as a one-thread kernel)
+            // compressor: the generator is inherently serial, far cheaper on a host core than as a
+            // one-thread kernel)
             py::gil_scoped_release nogil;
             uint32_t* p = reinterpret_cast<uint32_t*>(ptr);
             for (size_t i = 0; i < k; ++i) p[i] = (uint32_t)r.randint(0, high);

@@ -1,4 +1,4 @@
-// pybind11 surface of the sm_100a extension (module byteps_b200._cuda).
+// pybind11 surface of the sm_90a extension (module byteps_b200._cuda).
 // Tensors cross the boundary as raw device pointers + CUDA stream handles, so
 // this module needs no torch headers and rebuilds in seconds.
 #include <cuda_runtime_api.h>
@@ -52,7 +52,7 @@ PeerView make_view(const std::vector<uintptr_t>& data, const std::vector<uintptr
 }  // namespace
 
 PYBIND11_MODULE(_cuda, m) {
-  m.doc() = "byteps_b200 sm_100a kernels + symmetric memory";
+  m.doc() = "byteps_b200 sm_90a kernels + symmetric memory";
   m.attr("MAX_RANKS") = kMaxRanks;
   m.attr("MAX_BLOCKS") = kMaxBlocks;
   m.attr("SIG_BYTES") = kSigBytes;

@@ -80,7 +80,7 @@ void bind_cuda_ext(py::module_& m) {
       .def("stream", [](NcclManager& n, int ring) { return (uintptr_t)n.stream(ring); }, py::arg("ring") = 0)
       .def("num_rings", &NcclManager::num_rings);
 
-  // ---- tcgen05/TMEM/TMA push-pull variant
+  // ---- wgmma/TMA push-pull variant
   py::class_<UmmaMaps>(m, "UmmaMaps");
   m.def("make_umma_maps", [](const PeerView& pv, int wire, size_t off, size_t nelem) {
     UmmaMaps maps;

@@ -1,4 +1,4 @@
-// Host-side TMA tensor-map encoding for the tcgen05 push-pull variant.
+// Host-side TMA tensor-map encoding for the wgmma push-pull variant.
 #include <cuda.h>
 #include <cuda_runtime_api.h>
 

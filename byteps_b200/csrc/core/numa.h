@@ -2,9 +2,8 @@
 // only reaches NUMA through `numactl` in its launcher, /root/reference/launcher/launch.py:155-204).
 //
 // Why they exist: in colocated CPU-server mode the GPU DMAs a partition straight out of the server's
-// shared-memory store (pull by reference).  The device-timed copy profile (profiles/ps_mode_pipeline.md) shows
-// those copies running at 3-10 GB/s for runs of keys and at 30-45 GB/s for others on a 2-socket host, against
-// 52 GB/s for memory the copying process placed itself: the store of a key is first touched by whichever server
+// shared-memory store (pull by reference).  A device-timed copy profile on a 2-socket host showed those copies
+// several times slower for runs of keys than for memory the copying process placed itself: the store of a key is first touched by whichever server
 // thread handled its init push.  With BYTEPS_NUMA_AWARE=1 the worker announces the NUMA node of its GPU in the
 // init push, the server binds the key's store to that node and prefers an engine thread on it, and the worker
 // binds its own staging window the same way.  Everything here degrades to a no-op (returns false / -1) when the

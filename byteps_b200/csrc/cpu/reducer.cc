@@ -1,6 +1,6 @@
 #include "cpu/reducer.h"
 
-// x86 SIMD paths are optional: every kernel has a scalar loop behind it (aarch64 hosts - Grace-based Blackwell
+// x86 SIMD paths are optional: every kernel has a scalar loop behind it (aarch64 hosts - Grace Hopper
 // systems - and x86 without AVX2 build and run; define BPS_NO_X86_SIMD to force the scalar build for testing)
 #if (defined(__x86_64__) || defined(__i386__)) && defined(__AVX2__) && defined(__F16C__) && !defined(BPS_NO_X86_SIMD)
 #define BPS_X86_SIMD 1

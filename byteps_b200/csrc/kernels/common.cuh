@@ -1,4 +1,4 @@
-// Device-side helpers shared by the sm_100a kernels: 128-bit peer loads/stores,
+// Device-side helpers shared by the sm_90a kernels: 128-bit peer loads/stores,
 // bf16/fp16 packing, system-scope flag barriers over NVLink peer memory and the
 // NVLS multimem wrappers.
 #pragma once

@@ -9,7 +9,7 @@ namespace {
 
 constexpr int kThreads = 256;
 
-inline int grid_for(size_t n, int per_thread = 4, int cap = 148 * 8) {
+inline int grid_for(size_t n, int per_thread = 4, int cap = 132 * 8) {
   size_t b = (n + (size_t)kThreads * per_thread - 1) / ((size_t)kThreads * per_thread);
   if (b < 1) b = 1;
   if (b > (size_t)cap) b = cap;

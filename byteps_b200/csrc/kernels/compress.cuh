@@ -21,7 +21,7 @@ namespace bps {
 // corrected = g + ratio*err (fp32, written to `corrected`); acc[0] = sum|corrected|, acc[1] = sum corrected^2,
 // acc[2] = max|corrected|, computed with a fixed reduction order (bit-reproducible on every rank).
 // acc must hold kEfAccFloats floats (results + per-block partials).  err may be null (ratio ignored).
-constexpr int kEfAccFloats = 4 + 3 * 148 * 8;
+constexpr int kEfAccFloats = 4 + 3 * 132 * 8;
 cudaError_t launch_ef_correct(const void* g, int dtype, const float* err, float ratio, float* corrected, size_t n,
                               float* acc, cudaStream_t s);
 

@@ -2,8 +2,8 @@
 //
 // Round 1 ran the compressors as ~10 separate element-wise passes (EF correct, norm finalize,
 // pack, exchange, sum, recompress, unpack), read every peer's payload over NVLink element by
-// element and selected top-k with one global atomic per kept element: 1.06-1.09 ms for a 100 MB
-// gradient, slower than not compressing at all (0.60 ms).  Here:
+// element and selected top-k with one global atomic per kept element - slower than not compressing
+// at all.  Here:
 //
 //   * ONE producer pass reads the gradient (+ momentum + error feedback), writes the corrected
 //     value in place of the error state and emits the payload (sign words / first histogram) -
@@ -533,8 +533,8 @@ __global__ void __launch_bounds__(kSampleThreads) topk_sample_pick_kernel(size_t
 
 // Compaction: keys above the threshold take the first k - k_eq payload slots, ties take the rest.
 // Slots are handed out with ONE global atomic per block iteration (1024 elements): per-thread counts,
-// warp scan, block scan - a per-warp atomic on one address was the whole cost of this pass (160 us for
-// 25 M elements; same-address atomics retire about one per clock).  x_zero: the kept entries of x are
+// warp scan, block scan - a per-warp atomic on one address was the whole cost of this pass
+// (same-address atomics retire about one per clock).  x_zero: the kept entries of x are
 // zeroed, which IS the error-feedback update (the rest of the corrected tensor is already in place).
 __global__ void __launch_bounds__(kT) topk_compact_kernel(float* x, size_t n, uint32_t* pairs, int zero_kept,
                                                           TopkScratch* sc) {
@@ -815,7 +815,7 @@ __global__ void __launch_bounds__(kT) dither_sum_slots_kernel(const char* slots,
   }
 }
 
-inline int grid_for(size_t items, int cap = 148 * 8) {
+inline int grid_for(size_t items, int cap = 132 * 8) {
   size_t b = (items + kT - 1) / kT;
   if (b < 1) b = 1;
   if (b > (size_t)cap) b = cap;

@@ -13,7 +13,7 @@
 
 namespace bps {
 
-constexpr int kFusedMaxBlocks = 148 * 8;          // also the size of the per-block partial arrays
+constexpr int kFusedMaxBlocks = 132 * 8;          // also the size of the per-block partial arrays
 constexpr int kTopkScratchBytes = 4096 * 4 + 64 + 32768 * 4;
 
 // ---- onebit (+ nesterov momentum, + vanilla error feedback with the lr ratio) -------------------

@@ -60,7 +60,7 @@ __global__ void scale_inplace_kernel(T* x, size_t n, float alpha) {
 
 cudaError_t launch_scale_inplace(void* x, size_t n, int dtype, float alpha, cudaStream_t stream) {
   if (n == 0) return cudaSuccess;
-  const int grid = (int)((n + 1023) / 1024 < 1184 ? (n + 1023) / 1024 : 1184);
+  const int grid = (int)((n + 1023) / 1024 < 132 * 8 ? (n + 1023) / 1024 : 132 * 8);   // 8 CTAs per H100 SM
   if (dtype == 0) scale_inplace_kernel<float><<<grid, 256, 0, stream>>>((float*)x, n, alpha);
   else if (dtype == 1) scale_inplace_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>((__nv_bfloat16*)x, n, alpha);
   else if (dtype == 2) scale_inplace_kernel<__half><<<grid, 256, 0, stream>>>((__half*)x, n, alpha);
@@ -69,7 +69,7 @@ cudaError_t launch_scale_inplace(void* x, size_t n, int dtype, float alpha, cuda
 }
 
 cudaError_t launch_l2_flush(void* buf, size_t nbytes, uint32_t value, cudaStream_t stream) {
-  l2_flush_kernel<<<148 * 4, 512, 0, stream>>>(static_cast<uint4*>(buf), nbytes / 16, value);
+  l2_flush_kernel<<<132 * 4, 512, 0, stream>>>(static_cast<uint4*>(buf), nbytes / 16, value);
   return cudaGetLastError();
 }
 

@@ -1,4 +1,4 @@
-// Fused push-pull kernels for sm_100a (see pushpull.cuh for the contract).
+// Fused push-pull kernels for sm_90a (see pushpull.cuh for the contract).
 //
 // Geometry.  A wire UNIT is one 16-byte vector of the wire dtype W: E = 8
 // elements for bf16/fp16, E = 4 for fp32.  Consecutive lanes touch consecutive
@@ -118,8 +118,7 @@ __global__ void __launch_bounds__(512) pushpull_fused_opt_kernel(PeerView pv, co
 
 // ---- TMA-streamed variant of the fused optimizer kernel ---------------------------------------
 // The LSU kernel above holds the gradient AND the fp32 optimizer state of a unit in registers
-// (100-113 registers, one 512-thread CTA per SM, ~40 KB of loads in flight per SM: 0.75 of the
-// measured HBM copy bandwidth in ncu).  Here the state streams (master weights, momentum / Adam
+// (100-113 registers, one 512-thread CTA per SM, ~40 KB of loads in flight per SM).  Here the state streams (master weights, momentum / Adam
 // moments - contiguous fp32 arrays of this rank's shard) move through a shared-memory ring with
 // 1-D bulk copies: a producer thread prefetches `stages` tiles ahead (cp.async.bulk + mbarrier
 // complete_tx), consumers read the state from shared memory, update it in place and one thread

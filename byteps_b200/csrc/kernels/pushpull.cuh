@@ -1,4 +1,4 @@
-// Host-visible launch API of the fused push-pull kernels (sm_100a).
+// Host-visible launch API of the fused push-pull kernels (sm_90a).
 //
 // What the reference does with ncclReduceScatter + ncclAllGather (+ncclReduce/
 // ncclBroadcast tails) per <=4 MB partition, a host-side div_ and framework

@@ -442,7 +442,7 @@ __device__ __forceinline__ void reduce_phase(const PeerView& pv, size_t off, siz
 
 // NVLS-only variant with its own unroll: one multimem.ld_reduce per unit keeps 4 registers in flight per
 // unit (the P2P path needs 4 x peers), so many more units can be outstanding per thread - the in-switch
-// reduction is latency bound per CTA (one tile per ~3 us round trip), bytes in flight are what buys bandwidth.
+// reduction is latency bound per CTA (one tile per switch round trip), bytes in flight are what buys bandwidth.
 template <class W, int UNROLL, class Epi, class Sink>
 __device__ __forceinline__ void reduce_phase_nvls(const PeerView& pv, size_t off, size_t s0, size_t s1, Epi& epi,
                                                   Sink&& sink, CtaId id = CtaId()) {

@@ -1,4 +1,4 @@
-// Persistent descriptor-ring exchange kernel (sm_100a).
+// Persistent descriptor-ring exchange kernel (sm_90a).
 //
 // The reference moves every <=4 MB partition with its own NCCL calls, issued in groups of 4+4 by a
 // host thread that pops a priority queue with byte credits and tells the other ranks what it

@@ -1,22 +1,23 @@
-// tcgen05 / TMEM / TMA variant of the in-place push-pull (16-bit wire types).
+// wgmma / TMA variant of the in-place push-pull (16-bit wire types).
 //
 // Idea: the sum over peers IS a GEMM.  View a peer's slice of my shard as a
 // matrix X_p[128 rows][64 elems]; stack the peers along K:
 //
-//     D[128 x 64] (fp32, TMEM)  =  [ I | I | ... | I ] (128 x 128*P)  x  [ X_0 ; X_1 ; ... ; X_{P-1} ] (128*P x 64)
+//     D[128 x 64] (fp32, registers)  =  [ I | I | ... | I ] (128 x 128*P)  x  [ X_0 ; X_1 ; ... ; X_{P-1} ] (128*P x 64)
 //
 // The B operand is exactly what a 2-D TMA load with SWIZZLE_128B drops into
 // shared memory (MN-major canonical layout: 64 contiguous elements per K row,
 // 8-row swizzle atoms, SBO = 1024 B), so the NVLink traffic goes
-// peer HBM -> TMA -> smem -> tensor core without touching a register; the A
-// operand is a constant 128x128 identity kept in shared memory (eight 128x16
-// K-slices, reused for every peer).  The tensor pipe does the bf16->fp32
-// conversion and the fp32 accumulation at ~2 % of its capacity while the CUDA
-// cores only run the epilogue: tcgen05.ld of the fp32 tile (thread r owns row r =
-// 64 consecutive elements), scale, pack to 16 bit, bulk-store to every peer.
+// peer HBM -> TMA -> smem -> tensor core without touching a register.  The A
+// operand is the identity, passed as wgmma register fragments: the 64-row
+// M half h and the 16-row K slice j only meet on the diagonal (j = 4 h + warp),
+// so one warp of the warpgroup holds a 16 x 16 identity and the other three
+// hold zeros.  The tensor pipe does the bf16->fp32 conversion and the fp32
+// accumulation; the CUDA cores only run the epilogue: scale the fp32 tile,
+// pack to 16 bit, stage in smem, bulk-store to every peer.
 //
-// Warp roles (192 threads, 1 CTA/SM): warp 0 TMA producer, warp 1 MMA issuer +
-// TMEM allocator, warps 2-5 epilogue (TMEM lane quarter = warp % 4).
+// Warp roles (160 threads, 1 CTA/SM): warps 0-3 = the consumer warpgroup
+// (wgmma + epilogue), warp 4 = TMA producer.
 #include <cuda.h>
 
 #include "kernels/common.cuh"
@@ -27,27 +28,22 @@ namespace bps {
 
 namespace {
 
-constexpr int kRows = 128;                       // UMMA M
-constexpr int kCols = 64;                        // UMMA N = elements per row (128 B of 16-bit data)
+constexpr int kRows = 128;                       // tile rows = K rows per peer = 2 x wgmma M (64)
+constexpr int kCols = 64;                        // wgmma N = elements per row (128 B of 16-bit data)
 constexpr int kTileElems = kRows * kCols;        // 8192 elements
 constexpr int kTileBytes = kTileElems * 2;       // 16 KiB per peer per tile
 constexpr int kSlots = 6;                        // ring of peer tiles in flight per CTA
-constexpr int kThreadsUmma = 192;
-constexpr int kASliceBytes = kRows * 16 * 2;     // one 128 x 16 K-slice of the identity (4 KiB)
-constexpr int kTmemCols = 128;                   // two fp32 accumulators of 64 columns
+constexpr int kConsumerThreads = 128;            // one warpgroup
+constexpr int kThreadsUmma = kConsumerThreads + 32;
 
 struct UmmaSmem {
   uint64_t full[kSlots];
   uint64_t empty[kSlots];
-  uint64_t tmem_full[2];
-  uint64_t tmem_empty[2];
-  uint32_t tmem_base;
 };
 
-// smem layout: [UmmaSmem | pad to 1024][A: 8 x 4 KiB][ring: kSlots x 16 KiB (1024-aligned)][out: 16 KiB]
+// smem layout: [UmmaSmem | pad to 1024][ring: kSlots x 16 KiB (1024-aligned)][out: 16 KiB]
 constexpr size_t kSmemHeader = 1024;
-constexpr size_t kSmemA = kSmemHeader;
-constexpr size_t kSmemRing = kSmemA + 8 * kASliceBytes;
+constexpr size_t kSmemRing = kSmemHeader;
 constexpr size_t kSmemOut = kSmemRing + (size_t)kSlots * kTileBytes;
 constexpr size_t kSmemTotal = kSmemOut + kTileBytes + 1024;   // + slack for manual 1024 alignment
 
@@ -59,60 +55,44 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-// K-major, no swizzle: core matrix = 8 rows x 16 B; LBO = byte distance between the two K halves,
-// SBO = byte distance between 8-row groups along M
-__device__ __forceinline__ uint64_t make_desc_a(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);                 // start address
-  d |= (uint64_t)((2048u >> 4) & 0x3FFF) << 16;            // LBO = 2048 B
-  d |= (uint64_t)((128u >> 4) & 0x3FFF) << 32;             // SBO = 128 B
-  d |= (uint64_t)1 << 46;                                  // descriptor version (sm_100)
-  return d;                                                // layout_type 0 = no swizzle
-}
-// MN-major, SWIZZLE_128B: 64 contiguous elements per K row, 8-row atoms of 1024 B
+// sm_90 matrix descriptor, MN-major, SWIZZLE_128B: 64 contiguous elements per K row, 8-row atoms of 1024 B
 __device__ __forceinline__ uint64_t make_desc_b(uint32_t saddr) {
   uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
+  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);                 // start address
   d |= (uint64_t)1 << 16;                                  // LBO unused (single atom along N)
   d |= (uint64_t)((1024u >> 4) & 0x3FFF) << 32;            // SBO = 1024 B between 8-row groups along K
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;                                  // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                                  // layout type 1 = SWIZZLE_128B
   return d;
 }
-// kind::f16 instruction descriptor: D = F32, A/B = bf16 or f16, A K-major, B MN-major, M = 128, N = 64
-__host__ __device__ constexpr uint32_t make_idesc(bool bf16) {
-  return (1u << 4) | ((bf16 ? 1u : 0u) << 7) | ((bf16 ? 1u : 0u) << 10) | (0u << 15) | (1u << 16) |
-         ((uint32_t)(kCols >> 3) << 17) | ((uint32_t)(kRows >> 4) << 24);
-}
 
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a, uint64_t b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem),
-      "l"(a), "l"(b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// D[64 x 64] (+)= A[64 x 16] (registers) x B[16 x 64] (smem, MN-major: imm-trans-b = 1)
+template <bool BF16>
+__device__ __forceinline__ void wgmma_m64n64k16(float* d, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
+                                                uint64_t desc_b, uint32_t accumulate) {
+#define BPS_WGMMA_ASM(TYPE)                                                                                          \
+  asm volatile(                                                                                                      \
+      "{\n\t"                                                                                                        \
+      ".reg .pred p;\n\t"                                                                                            \
+      "setp.ne.b32 p, %37, 0;\n\t"                                                                                   \
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32." TYPE "." TYPE " "                                               \
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28," \
+      "%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1, 1;\n\t"                                                        \
+      "}"                                                                                                            \
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),             \
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),       \
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),     \
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])      \
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(desc_b), "r"(accumulate)                                            \
+      : "memory")
+  if (BF16)
+    BPS_WGMMA_ASM("bf16");
+  else
+    BPS_WGMMA_ASM("f16");
+#undef BPS_WGMMA_ASM
 }
 
 template <bool BF16>
@@ -123,11 +103,12 @@ __global__ void __launch_bounds__(kThreadsUmma, 1)
   // manual 1024-byte alignment (SWIZZLE_128B atoms)
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
   UmmaSmem* sm = reinterpret_cast<UmmaSmem*>(smem);
-  unsigned char* a_smem = smem + kSmemA;
   unsigned char* ring = smem + kSmemRing;
   unsigned char* out_smem = smem + kSmemOut;
   const int world = pv.world;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // warp index broadcast from lane 0: provably warp-uniform, so the role branches below are not divergent paths
+  // in which ptxas would have to serialize the wgmma instructions
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
 
   size_t b, e;
   shard_units(total_groups, world, pv.rank, &b, &e);
@@ -136,41 +117,17 @@ __global__ void __launch_bounds__(kThreadsUmma, 1)
   const size_t ntiles = (shard_elems + kTileElems - 1) / kTileElems;
 
   // ---- one-time setup
-  for (int i = threadIdx.x; i < 8 * kASliceBytes / 2; i += blockDim.x) {
-    // identity slice s: A_s[m][k] = (m == 16 s + k); K-major no-swizzle core-matrix layout
-    const int s = i / (kASliceBytes / 2), r = i % (kASliceBytes / 2);
-    const int khalf = r / (16 * 64), rem = r % (16 * 64);      // 2048 B per K half = 1024 elements
-    const int mgrp = rem / 64, in = rem % 64;                  // 128 B per 8-row group = 64 elements
-    const int mrow = in / 8, kin = in % 8;
-    const int m = mgrp * 8 + mrow, k = khalf * 8 + kin;
-    const uint16_t one = BF16 ? 0x3F80 : 0x3C00;
-    reinterpret_cast<uint16_t*>(a_smem)[i] = (m == 16 * s + k) ? one : (uint16_t)0;
-  }
   if (threadIdx.x == 0) {
     for (int s = 0; s < kSlots; ++s) {
       mbar_init(&sm->full[s], 1);
-      mbar_init(&sm->empty[s], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&sm->tmem_full[i], 1);
-      mbar_init(&sm->tmem_empty[i], 1);
+      mbar_init(&sm->empty[s], kConsumerThreads / 32);        // one arrival per consumer warp
     }
     mbar_fence_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sm->tmem_base)),
-                 "n"(kTmemCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  fence_proxy_async_smem();          // identity matrix (generic-proxy stores) -> visible to the tensor core
-  tc_fence_before();
   barrier_peers(pv, channel);        // __syncthreads inside: setup done AND every peer's input is ready
-  tc_fence_after();
   fence_proxy_async();
-  const uint32_t tmem_base = sm->tmem_base;
 
-  if (warp == 0) {
+  if (warp == kConsumerThreads / 32) {
     // ===== TMA producer
     if (lane == 0) {
       int s = 0;
@@ -187,70 +144,57 @@ __global__ void __launch_bounds__(kThreadsUmma, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer (one elected lane)
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(BF16);
-      int s = 0;
-      uint32_t phase = 0;
-      uint32_t it = 0;
-      for (size_t t = blockIdx.x; t < ntiles; t += gridDim.x, ++it) {
-        const uint32_t buf = it & 1, acc_phase = (it >> 1) & 1;
-        mbar_wait(&sm->tmem_empty[buf], acc_phase ^ 1);      // epilogue drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * kCols;
-        for (int p = 0; p < world; ++p) {
-          mbar_wait(&sm->full[s], phase);
-          tc_fence_after();
-          const uint32_t b_base = smem_u32(ring + (size_t)s * kTileBytes);
+  } else {
+    // ===== consumer warpgroup: wgmma into two 64 x 64 fp32 accumulators (rows 0-63 / 64-127 of the tile),
+    // then registers -> 16-bit -> smem -> bulk store to every peer
+    const int g = lane >> 2, q = lane & 3;
+    // identity fragment of this thread: a0 = a3 = (row g, cols 2q, 2q+1), a1 = a2 = 0
+    const uint32_t one = BF16 ? 0x3F80u : 0x3C00u;
+    const uint32_t ident = (g == 2 * q ? one : 0u) | ((g == 2 * q + 1 ? one : 0u) << 16);
+    int s = 0;
+    uint32_t phase = 0;
+    for (size_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+      float acc[2][32];
+      for (int p = 0; p < world; ++p) {
+        mbar_wait(&sm->full[s], phase);
+        const uint32_t b_base = smem_u32(ring + (size_t)s * kTileBytes);
+        wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {                       // K = 128 rows of this peer, 16 per MMA
-            const uint64_t da = make_desc_a(smem_u32(a_smem + j * kASliceBytes));
-            const uint64_t db = make_desc_b(b_base + j * 16 * 128);
-            umma_f16(d_tmem, da, db, idesc, (p | j) != 0);
-          }
-          umma_commit(&sm->empty[s]);                         // slot reusable once these MMAs retire
-          if (++s == kSlots) {
-            s = 0;
-            phase ^= 1;
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int w = 0; w < 4; ++w) {                       // K slice j = 4 h + w of this peer's 128 rows
+            const uint32_t a = warp == w ? ident : 0u;
+            wgmma_m64n64k16<BF16>(acc[h], a, 0u, 0u, a, make_desc_b(b_base + (4 * h + w) * 16 * 128),
+                                  (p | w) != 0);
           }
         }
-        umma_commit(&sm->tmem_full[buf]);                     // accumulator complete -> epilogue
+        wgmma_commit();
+        wgmma_wait_all();
+        if (lane == 0) mbar_arrive(&sm->empty[s]);            // slot reusable: this warp's MMAs have retired
+        if (++s == kSlots) {
+          s = 0;
+          phase ^= 1;
+        }
       }
-    }
-  } else {
-    // ===== epilogue warps 2..5: TMEM -> registers -> 16-bit -> smem -> bulk store to every peer
-    const int quarter = warp & 3;                             // TMEM lane quarter this warp may touch
-    const int row = quarter * 32 + lane;
-    uint32_t it = 0;
-    for (size_t t = blockIdx.x; t < ntiles; t += gridDim.x, ++it) {
-      const uint32_t buf = it & 1, acc_phase = (it >> 1) & 1;
-      mbar_wait(&sm->tmem_full[buf], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + buf * kCols + ((uint32_t)(quarter * 32) << 16);
-      uint32_t packed[32];
+      // the previous tile's bulk stores must have finished reading out_smem
+      if (threadIdx.x == 0) bulk_wait_read<0>();
+      named_bar_sync(1, kConsumerThreads);
+      // accumulator layout: acc[h][4c + i] = row 64 h + 16 warp + g + 8 (i >> 1), column 8 c + 2 q + (i & 1)
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        uint32_t r[32];
-        tmem_ld32(taddr + h * 32, r);
+        unsigned char* row0 = out_smem + (size_t)(64 * h + 16 * warp + g) * 128 + q * 4;
 #pragma unroll
-        for (int k = 0; k < 16; ++k) {
-          float x = __uint_as_float(r[2 * k]) * scale, y = __uint_as_float(r[2 * k + 1]) * scale;
-          packed[h * 16 + k] = BF16 ? f2_to_bf16x2(x, y) : f2_to_f16x2(x, y);
+        for (int c = 0; c < 8; ++c) {
+          const float* v = &acc[h][4 * c];
+          const uint32_t lo = BF16 ? f2_to_bf16x2(v[0] * scale, v[1] * scale) : f2_to_f16x2(v[0] * scale, v[1] * scale);
+          const uint32_t hi = BF16 ? f2_to_bf16x2(v[2] * scale, v[3] * scale) : f2_to_f16x2(v[2] * scale, v[3] * scale);
+          *reinterpret_cast<uint32_t*>(row0 + c * 16) = lo;
+          *reinterpret_cast<uint32_t*>(row0 + 8 * 128 + c * 16) = hi;
         }
       }
-      tc_fence_before();
-      // the previous tile's bulk stores must have finished reading out_smem
-      if (threadIdx.x == 64) bulk_wait_read<0>();
-      named_bar_sync(1, 128);
-      if (threadIdx.x == 64) mbar_arrive(&sm->tmem_empty[buf]);   // accumulator is in registers: release it
-      unsigned char* dst = out_smem + (size_t)row * 128;
-#pragma unroll
-      for (int c = 0; c < 8; ++c)   // static register indices (a rotated order would spill `packed` to local memory)
-        sts16(dst + c * 16, Vec16{packed[c * 4], packed[c * 4 + 1], packed[c * 4 + 2], packed[c * 4 + 3]});
       fence_proxy_async_smem();
-      named_bar_sync(1, 128);
-      if (threadIdx.x == 64) {
+      named_bar_sync(1, kConsumerThreads);
+      if (threadIdx.x == 0) {
         const size_t done = t * (size_t)kTileElems;
         const size_t left = shard_elems - done;
         const uint32_t bytes = (uint32_t)((left < (size_t)kTileElems ? left : (size_t)kTileElems) * 2);
@@ -262,16 +206,12 @@ __global__ void __launch_bounds__(kThreadsUmma, 1)
         bulk_commit();
       }
     }
-    if (threadIdx.x == 64) {
+    if (threadIdx.x == 0) {
       bulk_wait<0>();
       fence_proxy_async();
     }
   }
-  tc_fence_before();
   barrier_peers(pv, channel);
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(kTmemCols) : "memory");
-  }
 }
 
 }  // namespace

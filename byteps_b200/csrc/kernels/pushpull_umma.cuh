@@ -1,4 +1,4 @@
-// tcgen05/TMEM/TMA variant of the in-place push-pull (see pushpull_umma.cu).
+// wgmma/TMA variant of the in-place push-pull (see pushpull_umma.cu).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>

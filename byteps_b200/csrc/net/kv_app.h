@@ -334,7 +334,7 @@ class KVServer : public SimpleApp {
         if (base && res.vals.size() <= req.shm_len) {
           // the reference hands this copy to BYTEPS_IPC_COPY_NUM_THREADS async copy threads
           // (rdma_transport.h:577-644); one memcpy of a 4 MB partition per response was THE bottleneck of the
-          // colocated CPU-server path (11 GB/s per worker on a 128-thread host)
+          // colocated CPU-server path
           const auto t0 = std::chrono::steady_clock::now();
           ipc_copy((char*)base + req.shm_offset, res.vals.data(), res.vals.size());
           via_shm = true;

@@ -6,12 +6,30 @@
 #include <unistd.h>
 
 #include <algorithm>
+#include <cstddef>
+#include <cstdio>
 #include <cstring>
 
 #include "core/env.h"
 #include "core/log.h"
 
 namespace bps {
+
+// Address of a local socket.  A path that does not fit sun_path (a deep BYTEPS_SOCKET_PATH) would be truncated,
+// and truncated paths of different ranks collide; such a path is replaced by an abstract-namespace name derived
+// from a hash of the whole path, which every rank computes alike.
+static socklen_t unix_addr(const std::string& path, sockaddr_un* a) {
+  memset(a, 0, sizeof(*a));
+  a->sun_family = AF_UNIX;
+  if (path.size() < sizeof(a->sun_path)) {
+    memcpy(a->sun_path, path.data(), path.size());
+    return (socklen_t)sizeof(*a);
+  }
+  uint64_t h = 1469598103934665603ull;   // FNV-1a
+  for (unsigned char c : path) h = (h ^ c) * 1099511628211ull;
+  const int n = snprintf(a->sun_path + 1, sizeof(a->sun_path) - 1, "byteps_local_%016llx", (unsigned long long)h);
+  return (socklen_t)(offsetof(sockaddr_un, sun_path) + 1 + n);
+}
 
 LocalComm::LocalComm(int local_rank, const std::vector<int>& members, const std::string& dir, const std::string& suffix,
                      bool start_listening)
@@ -24,10 +42,8 @@ LocalComm::LocalComm(int local_rank, const std::vector<int>& members, const std:
   std::string p = path_of(rank_);
   unlink(p.c_str());
   sockaddr_un a;
-  memset(&a, 0, sizeof(a));
-  a.sun_family = AF_UNIX;
-  strncpy(a.sun_path, p.c_str(), sizeof(a.sun_path) - 1);
-  BPS_CHECK_EQ(bind(fd_, (sockaddr*)&a, sizeof(a)), 0) << "bind(" << p << ") failed: " << strerror(errno);
+  const socklen_t alen = unix_addr(p, &a);
+  BPS_CHECK_EQ(bind(fd_, (sockaddr*)&a, alen), 0) << "bind(" << p << ") failed: " << strerror(errno);
   // a receive timeout lets blocked readers notice shutdown (reference: 3 s SO_RCVTIMEO)
   timeval tv{0, 200000};
   setsockopt(fd_, SOL_SOCKET, SO_RCVTIMEO, &tv, sizeof(tv));
@@ -49,11 +65,9 @@ std::string LocalComm::path_of(int r) const { return dir_ + "/socket_" + suffix_
 
 static bool send_msg(int fd, const std::string& path, const LocalMsg& m) {
   sockaddr_un a;
-  memset(&a, 0, sizeof(a));
-  a.sun_family = AF_UNIX;
-  strncpy(a.sun_path, path.c_str(), sizeof(a.sun_path) - 1);
+  const socklen_t alen = unix_addr(path, &a);
   for (int attempt = 0; attempt < 2000; ++attempt) {
-    ssize_t r = sendto(fd, &m, sizeof(m), 0, (sockaddr*)&a, sizeof(a));
+    ssize_t r = sendto(fd, &m, sizeof(m), 0, (sockaddr*)&a, alen);
     if (r == (ssize_t)sizeof(m)) return true;
     if (errno == ENOENT || errno == ECONNREFUSED || errno == EAGAIN || errno == ENOBUFS) {
       usleep(1000);   // the peer has not bound its socket yet / queue full

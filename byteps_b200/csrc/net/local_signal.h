@@ -5,7 +5,7 @@
 // {src, signal, key}, the root runs a listen thread that turns *_READY signals
 // into ReadyTable increments, and the root can broadcast DO_* commands that the
 // other ranks receive in order.  In the reference this protocol gates every
-// NCCL call; on the B200 data path readiness is detected by flags in peer
+// NCCL call; on the H100 data path readiness is detected by flags in peer
 // device memory instead (common.cuh barrier_peers, the ring kernel's per-slot
 // generations), and launch order is enforced on the device (ring scheduler
 // warp) or by BYTEPS_STRICT_ORDER.  The protocol is used where the data really

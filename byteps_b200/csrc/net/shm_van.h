@@ -1,4 +1,4 @@
-// ShmVan: a socket-free transport for jobs whose nodes all live on ONE host (an 8xB200 box running scheduler,
+// ShmVan: a socket-free transport for jobs whose nodes all live on ONE host (an 8xH100 box running scheduler,
 // servers and workers side by side).  It plays the role ps-lite's RDMAVan + IPCTransport play between hosts
 // (/root/reference/3rdparty/ps-lite/src/rdma_van.h:26-975, rdma_transport.h:513-712): one-sided writes into
 // memory the receiver registered up front, completion by polling, no kernel on the data path - with POSIX

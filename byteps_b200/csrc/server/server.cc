@@ -92,7 +92,7 @@ static char* page_alloc(size_t n) {
 SumServer::SumServer(net::Postoffice* po, const ServerConfig& cfg, int app_id)
     : po_(po), cfg_(cfg),
       // threads of ONE summation: 1 on small hosts (the engine threads already use the cores), 4 from 64 hardware
-      // threads up (a 4 MB partition merged by one thread was 1-1.5 ms of the colocated path)
+      // threads up (one thread merging a 4 MB partition dominated the colocated path)
       reducer_((int)env_int("BYTEPS_SERVER_OMP_THREADS", std::thread::hardware_concurrency() >= 64 ? 4 : 1)) {
   pushers_ = cfg.pushers_per_key > 0 ? cfg.pushers_per_key : po->num_workers();
   inline_bytes_ = (size_t)std::max<long long>(0, env_int("BYTEPS_SERVER_INLINE_BYTES", 16384));

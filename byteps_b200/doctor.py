@@ -49,7 +49,7 @@ def collect() -> dict:
             gpus.append({"index": i, "name": p.name, "sm": "%d.%d" % (p.major, p.minor),
                          "memory_gb": round(p.total_memory / 2 ** 30, 1), "sms": p.multi_processor_count,
                          "peer_access": peers})
-        info["sm_100_family"] = all(g["sm"].startswith("10.") for g in gpus) if gpus else False
+        info["sm_90_family"] = all(g["sm"] == "9.0" for g in gpus) if gpus else False
     info["gpus"] = gpus
     from .config import Config
 
@@ -110,8 +110,8 @@ def main(argv=None) -> int:
     for g in info.get("gpus", []):
         print("  GPU %d          : %s, sm_%s, %.0f GB, %d SMs, peer access to %s" % (
             g["index"], g["name"], g["sm"].replace(".", ""), g["memory_gb"], g["sms"], g["peer_access"] or "nobody"))
-    if info.get("gpus") and not info.get("sm_100_family"):
-        print("  WARNING        : the kernels are built for sm_100a only; they will not load on these GPUs")
+    if info.get("gpus") and not info.get("sm_90_family"):
+        print("  WARNING        : the kernels are built for sm_90a only; they will not load on these GPUs")
     w = info["world"]
     print("  topology       : rank %d of %d (local %d of %d), %d worker box(es), %d server(s)%s" % (
         w["rank"], w["size"], w["local_rank"], w["local_size"], w["num_worker"], w["num_server"],

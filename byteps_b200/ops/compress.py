@@ -128,7 +128,7 @@ class GpuCompressor:
             self.scale2 = torch.empty(4, **f32)
             self.corrected = torch.empty(n, **f32)
             self.sum = torch.empty(n, **f32)
-            self.acc = torch.zeros(4 + 3 * 148 * 8, **f32)   # results + per-block partials (kEfAccFloats)
+            self.acc = torch.zeros(4 + 3 * 132 * 8, **f32)   # results + per-block partials (kEfAccFloats)
         self.blocks = max(1, min(128, (self.wire_bytes + 65535) // 65536))
         self.payload = ctx.arena[self.off:self.off + self.payload_bytes]
 

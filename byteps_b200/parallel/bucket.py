@@ -1,6 +1,6 @@
 """Zero-copy bucketed gradient synchronisation over symmetric memory.
 
-This is the B200-first replacement for the reference's per-parameter
+This is the H100-first replacement for the reference's per-parameter
 ``push_pull_async_inplace`` hooks (/root/reference/byteps/torch/__init__.py:117-158)
 and its per-<=4MB-partition NCCL reduce-scatter/all-gather launches
 (core_loops.cc:190-269): gradients LIVE in a peer-mapped arena (``p.grad`` are
@@ -34,6 +34,9 @@ def _env_int(name, default):
 
 def _pad8(n: int) -> int:
     return (n + 7) // 8 * 8
+
+
+REDUCE_ENGINES = ("auto", "nvls", "lsu", "tma", "wgmma")
 
 
 def _strided_view(flat: torch.Tensor, p: torch.Tensor, offset: int) -> torch.Tensor:
@@ -101,6 +104,10 @@ class BucketedGradSync:
         self.engine = engine
         self.world, self.rank = engine.size, engine.rank
         self.fused = fused                     # None | "sgd" | "adam" | "adamw"
+        reduce_engine = os.environ.get("BYTEPS_REDUCE_ENGINE", "auto").lower()
+        if reduce_engine not in REDUCE_ENGINES:
+            raise ValueError("BYTEPS_REDUCE_ENGINE=%s: expected one of %s (the tensor-core engine of sm_90a is 'wgmma')"
+                             % (reduce_engine, "|".join(REDUCE_ENGINES)))
         self.average = average
         self.bpps = backward_passes_per_step
         self.bucket_bytes = bucket_bytes or _env_int("BYTEPS_BUCKET_BYTES", 16 << 20)
@@ -184,15 +191,14 @@ class BucketedGradSync:
         self._trace_spans = []
         # which engine moves the NVLink bytes of plain (unfused) buckets:
         #   auto/nvls: multimem.ld_reduce/st when available, else LSU P2P; lsu: force P2P loads/stores;
-        #   tma: cp.async.bulk ring; tcgen05: TMA + tensor-core reduction with a TMEM accumulator
-        self._reduce_engine = os.environ.get("BYTEPS_REDUCE_ENGINE", "auto").lower()
+        #   tma: cp.async.bulk ring; wgmma: TMA + tensor-core reduction with a register accumulator
+        self._reduce_engine = reduce_engine
         # fused optimizer kernels: "tma" streams the fp32 state through shared memory with bulk copies,
         # "lsu" keeps it in registers (also used whenever the gradients need a wire cast)
         self._fused_engine = os.environ.get("BYTEPS_FUSED_ENGINE", "auto").lower()
         if self._fused_engine == "auto":
-            # measured in situ (BERT-large AdamW, bench.py): one GPU 23.07 ms/step (tma, 128 CTAs) vs 23.33 (lsu);
-            # two GPUs 23.38 vs 23.11 - within noise, so the register kernel (validated on 8 GPUs) stays the
-            # multi-GPU default and the TMA kernel (0.92/0.88 vs 0.75/0.77 of the HBM roofline alone) runs solo
+            # the TMA kernel keeps more bytes in flight per SM (shared-memory ring instead of registers) and runs
+            # solo; the register kernel stays the multi-GPU default and handles every wire cast
             self._fused_engine = "tma" if self.world == 1 else "lsu"
         # CTAs of the TMA variant: its bytes in flight live in shared memory, so a fraction of the SMs
         # saturates HBM/NVLink and the rest stays free for the backward kernels it overlaps with
@@ -414,8 +420,8 @@ class BucketedGradSync:
                                   nvls, cs.cuda_stream)
         elif wire == b.dtype:
             eng_kind = self._reduce_engine
-            if eng_kind == "tcgen05" and b.dtype in (torch.bfloat16, torch.float16) and world <= 8:
-                # tensor-core reduction: TMA-fed [I|..|I] x [X_0;..;X_{P-1}] with a TMEM accumulator
+            if eng_kind == "wgmma" and b.dtype in (torch.bfloat16, torch.float16) and world <= 8:
+                # tensor-core reduction: TMA-fed [I|..|I] x [X_0;..;X_{P-1}] accumulated in registers
                 maps = self._umma_maps.get(b.index)
                 if maps is None:
                     maps = cu.make_umma_maps(view, wire_code(wire), b.grad_off, b.numel)

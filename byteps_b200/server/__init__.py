@@ -32,7 +32,7 @@ def run(role=None):
         os.environ.get("BYTEPS_LOG_LEVEL", "WARNING").upper(), 3)
     core.set_log_level(lvl)
     # BYTEPS_SERVER_NUMA_NODE=N: run the whole server (its threads are created below) on NUMA node N and prefer its
-    # memory - the socket the GPUs hang off when workers DMA out of the server's store (profiles/ps_mode_pipeline.md);
+    # memory - the socket the GPUs hang off when workers DMA out of the server's store;
     # the same as starting it under `numactl --cpunodebind=N --preferred=N`
     node = os.environ.get("BYTEPS_SERVER_NUMA_NODE", "")
     if role == "server" and node not in ("", "-1"):

@@ -4,7 +4,7 @@
 
 TensorFlow is not part of this image; the module binds to whatever ``tensorflow`` is importable
 and is exercised in tests/test_plugins.py against a minimal stand-in.  The exchange itself runs in
-the shared engine (ops.py), so TF gradients on a B200 ride the same NVLink kernels as torch ones.
+the shared engine (ops.py), so TF gradients on an H100 ride the same NVLink kernels as torch ones.
 """
 from __future__ import annotations
 

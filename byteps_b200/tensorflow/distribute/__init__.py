@@ -9,7 +9,7 @@ processes with ``_push_pull``.  Here the same behaviour is built on TensorFlow's
 * ``BytepsCrossDeviceOps`` subclasses ``tf.distribute.CrossDeviceOps`` and implements the three abstract
   methods (``reduce_implementation``, ``batch_reduce_implementation``, ``broadcast_implementation``): local
   replicas are combined by a ``tf.distribute.ReductionToOneDevice`` (or whatever ``local_ops`` is given),
-  then each component is exchanged through the shared engine - on a B200 that is the NVLink push-pull
+  then each component is exchanged through the shared engine - on an H100 that is the NVLink push-pull
   kernel, reached zero-copy through DLPack (ops.py).
 * ``BytepsAllReduce(num_packs)`` keeps the reference's constructor; ``num_packs`` groups the tensors of a
   ``batch_reduce`` into that many concatenated exchanges (1 = everything in one launch, 0 = one per tensor).

@@ -9,7 +9,7 @@ Parity: /root/reference/byteps/torch/__init__.py:23-466.  Same entry points:
 
 What is different underneath: on CUDA the optimizer does not issue one
 push_pull per parameter.  Gradients live in a symmetric NVLink-mapped arena and
-are exchanged bucket by bucket by one fused sm_100a kernel each
+are exchanged bucket by bucket by one fused sm_90a kernel each
 (:mod:`byteps_b200.parallel.bucket`); with ``fused_update=True`` the kernel also
 applies the SGD/Adam step on fp32 master weights and all-gathers the new
 parameters instead of the gradients.

@@ -4,7 +4,7 @@ Parity: /root/reference/byteps/misc/imagenet18/__init__.py:39-382
 (``DistributedOptimizer`` for fp16 models: fp16 params + fp32 master copy,
 gradients pushed with priority = order of first appearance, per-parameter SGD
 on the master as each handle completes, copy back to fp16, static/dynamic loss
-scale).  On B200 this is the *default shape* of the fused path: the exchange
+scale).  On H100 this is the *default shape* of the fused path: the exchange
 kernel reads bf16/fp16 gradients, accumulates in fp32, divides by
 loss_scale*size, updates the fp32 master shard and writes the half-precision
 weights to every rank - all in one kernel per bucket.

@@ -1,14 +1,14 @@
 #!/usr/bin/env python
 """Build / install byteps_b200.
 
-    python setup.py build_ext --inplace      # compile _core (g++) and _cuda (nvcc sm_100a) next to the sources
+    python setup.py build_ext --inplace      # compile _core (g++) and _cuda (nvcc sm_90a) next to the sources
     pip install --no-build-isolation -e .     # editable install; the .so files stay in-tree
 
 The reference's setup.py (/root/reference/setup.py:177-1075) builds ps-lite with make (downloading
 ZeroMQ), then one extension per framework against TH/THC, TF and MXNet headers.  Here there are two
 framework-independent modules driven by byteps_b200/_build.py: `_core` (C++17 runtime: registry,
 scheduler, reducer, compressors, transport, server, PS worker; also linked as libbyteps_b200.so for the C API) and
-`_cuda` (sm_100a kernels, symmetric memory, NCCL baseline manager), plus `_torch_ops` (the native torch adapter,
+`_cuda` (sm_90a kernels, symmetric memory, NCCL baseline manager), plus `_torch_ops` (the native torch adapter,
 pybind over at::Tensor); the other framework front ends are python over the same engine.
 Environment: BYTEPS_WITHOUT_CUDA=1 skips the CUDA module (CPU-only boxes without nvcc).
 """
@@ -60,7 +60,7 @@ class BuildNative(Command):
 setup(
     name="byteps_b200",
     version="0.1.0",
-    description="Blackwell-native gradient synchronisation with the capabilities of bytedance/byteps",
+    description="Hopper-native gradient synchronisation with the capabilities of bytedance/byteps",
     packages=find_packages(include=["byteps_b200", "byteps_b200.*"]),
     package_data={"byteps_b200": ["*.so", "csrc/*/*"]},
     scripts=["bin/bpslaunch"],

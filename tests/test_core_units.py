@@ -848,6 +848,17 @@ def test_host_local_reduce_three_ranks(tmp_path):
     run_workers(_host_reduce_rank, world=3, args=("unit%d" % os.getpid(), str(tmp_path)), timeout=120)
 
 
+def test_host_local_reduce_deep_socket_dir(tmp_path):
+    """A socket directory too deep for sun_path (108 bytes) must not make the ranks' socket names collide."""
+    import os
+
+    from _mp import run_workers
+
+    d = tmp_path / ("d" * 120)
+    d.mkdir()
+    run_workers(_host_reduce_rank, world=3, args=("deep%d" % os.getpid(), str(d)), timeout=120)
+
+
 def _host_reduce_timeouts(rank, world, tag, tmp):
     import time
 
@@ -883,3 +894,15 @@ def test_host_local_reduce_timeouts_do_not_hang(tmp_path):
     from _mp import run_workers
 
     run_workers(_host_reduce_timeouts, world=2, args=("tmo%d" % os.getpid(), str(tmp_path)), timeout=120)
+
+
+def test_unknown_reduce_engine_is_rejected(monkeypatch):
+    """A BYTEPS_REDUCE_ENGINE the exchange does not know (e.g. the former 'tcgen05') is an error, not a silent
+    fall-back to the default engine; it is rejected before any parameter is touched."""
+    from types import SimpleNamespace
+
+    from byteps_b200.parallel.bucket import BucketedGradSync
+
+    monkeypatch.setenv("BYTEPS_REDUCE_ENGINE", "tcgen05")
+    with pytest.raises(ValueError, match="wgmma"):
+        BucketedGradSync(SimpleNamespace(size=1, rank=0), [])

@@ -1,4 +1,4 @@
-"""Numerics of the sm_100a push-pull kernels against plain PyTorch fp32 references.
+"""Numerics of the sm_90a push-pull kernels against plain PyTorch fp32 references.
 
 Multi-peer behaviour is exercised on ONE GPU with `VirtualCluster`: N virtual
 ranks, N concurrent kernels on N streams, same flag protocol and peer-pointer
@@ -98,8 +98,8 @@ def test_inplace_pushpull_tma_virtual(world, dt):
 @pytest.mark.parametrize("world", [1, 2, 8])
 @pytest.mark.parametrize("dt", ["bf16", "f16"])
 def test_inplace_pushpull_umma_virtual(world, dt):
-    """tcgen05 variant: the peer sum computed by the tensor core as [I|I|...|I] x [X_0;...;X_{P-1}]
-    with TMA-fed operands and a TMEM accumulator must match the fp32 reference."""
+    """wgmma variant: the peer sum computed by the tensor core as [I|I|...|I] x [X_0;...;X_{P-1}]
+    with TMA-fed operands and a register accumulator must match the fp32 reference."""
     from byteps_b200.comm.symm import VirtualCluster
 
     cu = _cu()

@@ -1,15 +1,15 @@
 #!/usr/bin/env bash
-# compute-sanitizer pass over the single-rank GPU kernel tests (run on a B200 box, e.g. through gpurun):
+# compute-sanitizer pass over the single-rank GPU kernel tests (run on an H100):
 #   tools/gpu_sanitize.sh memcheck|racecheck|synccheck|initcheck [all]
 # Only world=1 cases are selected: the multi-rank kernels spin on each other's flags and the sanitizer serialises
 # kernel launches, so virtual-cluster tests would dead-lock under it (the spin watchdog would trap).
-# Default: one case per kernel family (what round 2 ran: 8 passed, 0 errors, 9 s under memcheck,
-# profiles/logs/sanitizer_memcheck*.log); `all` selects every world-1 case (several minutes).
+# Default: one case per kernel family; `all` selects every world-1 case (several minutes).
 set -euo pipefail
 TOOL=${1:-memcheck}
 ROOT=$(cd "$(dirname "$0")/.." && pwd)
 cd "$ROOT"
-mkdir -p gpurun_out
+OUT=${SANITIZER_OUT:-/tmp/byteps_b200_sanitizer}   # logs go outside the tree
+mkdir -p "$OUT"
 if [ "${2:-}" = "all" ]; then
   SEL=(tests/test_gpu_kernels.py tests/test_gpu_ring.py tests/test_gpu_compress.py -k "1] and not multigpu")
 else
@@ -23,6 +23,6 @@ else
        "tests/test_gpu_compress.py::test_gpu_compressor_matches_cpu_reference[kw1-1]")
 fi
 timeout 1200 compute-sanitizer --tool "$TOOL" --error-exitcode 3 \
-  --log-file gpurun_out/sanitizer_"$TOOL".log \
+  --log-file "$OUT"/sanitizer_"$TOOL".log \
   python -m pytest -q -p no:cacheprovider --timeout 600 "${SEL[@]}" || true
-tail -30 gpurun_out/sanitizer_"$TOOL".log
+tail -30 "$OUT"/sanitizer_"$TOOL".log
