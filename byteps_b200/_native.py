@@ -57,11 +57,9 @@ _torch_ops = None
 
 
 def torch_ops():
-    """The native torch adapter (push_pull on at::Tensor); None when it is disabled
-    (BYTEPS_NATIVE_OPS=0) - building it needs the torch headers of the running interpreter."""
+    """The native torch adapter (push_pull on at::Tensor).  Fails loudly like cuda() - building it
+    needs the torch headers of the running interpreter."""
     global _torch_ops
-    if os.environ.get("BYTEPS_NATIVE_OPS", "1") in ("0", ""):
-        return None
     if _torch_ops is None:
         with _lock:
             if _torch_ops is None:

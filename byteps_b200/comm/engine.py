@@ -18,16 +18,16 @@ from __future__ import annotations
 
 import threading
 from dataclasses import dataclass, field
-from typing import Dict, List, Optional
+from typing import Dict, Optional
 
 import torch
 
 from .. import _native
 from ..config import Config
-from .symm import SymmContext, pick_blocks, wire_code
+from .symm import SymmContext
 
 _CORE_DT = None
-_ES = {torch.float32: 4, torch.bfloat16: 2, torch.float16: 2}
+_SYMM_DTYPES = (torch.float32, torch.bfloat16, torch.float16)    # what the symmetric-memory kernels reduce
 
 
 def core_dtype(dtype: torch.dtype) -> int:
@@ -44,22 +44,12 @@ def core_dtype(dtype: torch.dtype) -> int:
         raise ValueError("Tensor type %s is not supported." % dtype)
 
 
-class _Part:
-    """One partition of an enqueued tensor (raw pointers: no tensor views on the hot path)."""
-    __slots__ = ("key", "src", "dst", "numel", "handle", "average", "nbytes", "dtype", "device")
-
-    def __init__(self, key, src, dst, numel, handle, average, nbytes, dtype, device):
-        self.key, self.src, self.dst, self.numel = key, src, dst, numel
-        self.handle, self.average, self.nbytes, self.dtype, self.device = handle, average, nbytes, dtype, device
-
-
 @dataclass
 class _HandleState:
     tensor: torch.Tensor
     output: torch.Tensor
     name: str
     average: bool
-    pending_parts: int = 0
     done_event: Optional[torch.cuda.Event] = None
     work: list = field(default_factory=list)    # torch.distributed Work objects
     post: list = field(default_factory=list)    # callables run at synchronize
@@ -77,9 +67,6 @@ class PushPullEngine:
         self.timeline = self.core.Timeline()
         self.timeline.configure(cfg.trace_on, cfg.trace_start_step, cfg.trace_end_step, cfg.trace_dir, cfg.local_rank)
         self.telemetry = self.core.Telemetry(cfg.telemetry_on, 10.0)
-        credits = cfg.scheduling_credit * cfg.partition_bound() if cfg.scheduling_credit > 0 else 0
-        self.queue = self.core.ScheduledQueue(self.core.REDUCE, True, credits)
-        self._parts: Dict[int, List[_Part]] = {}   # key -> FIFO of parts sharing the key
         self._handles: Dict[int, _HandleState] = {}
         self._next_handle = 0
         self._lock = threading.RLock()
@@ -88,17 +75,10 @@ class PushPullEngine:
         self.rank, self.size = cfg.rank, cfg.size
         self.symm: Optional[SymmContext] = None
         self.comm_stream = None
-        self._stage_cursor = 0
-        self._seg_ring = []
-        self._seg_slot = 0
-        self._prev_window = None
-        self._part_cache: Dict[str, tuple] = {}
-        self._flush_device = None
-        self._last_waited = None
         self._native_meta: Dict[int, tuple] = {}
         self._trace_native = bool(cfg.trace_on or cfg.debug_sample_tensor)
         self._launches = 0         # kernels of OURS launched (bench 'gpu_launches'), see the `launches` property
-        self._native = None        # csrc/torch/native_ops.cc: the per-tensor push_pull path without python
+        self._native = None        # csrc/torch/native_ops.cc: the per-tensor symmetric-memory push_pull
         self._compress_kwargs: Dict[str, Dict[str, str]] = {}   # per-tensor compressor config (declare kwargs)
         self._gpu_compressors: Dict[str, object] = {}
         self._compress_ctx: Optional[SymmContext] = None
@@ -138,8 +118,6 @@ class PushPullEngine:
         credit queue -> fused pack+exchange+unpack launches, with cudaStreamWaitEvent readiness and native
         handles (reference: byteps/torch/ops.cc:54-135, ready_event.cc, handle_manager.cc)."""
         mod = _native.torch_ops()
-        if mod is None:
-            return
         import os as _os
 
         cfg, ctx = self.cfg, self.symm
@@ -165,7 +143,7 @@ class PushPullEngine:
 
     def _auto_name(self) -> str:
         self._noname += 1
-        return "byteps.push_pull.noname.%d" % self._noname
+        return "push_pull.noname.%d" % self._noname
 
     # ------------------------------------------------------------------ gradient compression config
     def set_compression(self, name: str, kwargs: Optional[dict]):
@@ -238,59 +216,38 @@ class PushPullEngine:
     # ------------------------------------------------------------------ API
     def push_pull_async(self, tensor: torch.Tensor, output: torch.Tensor, average: bool, name: Optional[str],
                         version: int = 0, priority: int = 0, flush: bool = True) -> int:
-        if self._native is not None and name is not None:
-            fast = self._fast_push_pull(tensor, output, average, name, version, priority, flush)
-            if fast is not None:
-                return fast
         if not tensor.is_contiguous() or not output.is_contiguous():
             raise ValueError("Tensor is required to be contiguous.")
         core_dtype(tensor.dtype)  # validates dtype
-        name = ("byteps." + name) if name else self._auto_name()
-        if (self._native is None and self.backend == "symm" and tensor.is_cuda and self.symm is None
-                and tensor.dtype in _ES):
-            self._ensure_symm(tensor.device)           # first CUDA push_pull: map the arena, build the adapter
-            fast = self._fast_push_pull(tensor, output, average, name[7:], version, priority, flush)
-            if fast is not None:
-                return fast
+        name = "byteps." + (self._auto_name() if name is None else name)
+        nbytes = tensor.numel() * tensor.element_size()
+        symm = self.backend == "symm" and tensor.is_cuda and tensor.dtype in _SYMM_DTYPES and tensor.numel() > 0
+        if symm and not (name in self._compress_kwargs and nbytes >= self.cfg.min_compress_bytes):
+            # the native adapter: declare -> partition -> priority/credit queue -> fused launches
+            self._ensure_symm(tensor.device)
+            h = self._native.try_push_pull_async(tensor, output, average, name[7:], priority, version, flush)
+            if h < 0:
+                raise ValueError("push_pull of a CUDA tensor needs a CUDA output of the same dtype and size")
+            if self._trace_native:
+                self._native_meta[h] = (name, self.core.now_us())
+            return -(h + 1)          # handles of the native adapter are negative on this side
         with self._lock:
             self.registry.declare(name)
             h = self._next_handle
             self._next_handle += 1
             st = _HandleState(tensor, output, name, average, start_us=self.core.now_us())
             self._handles[h] = st
-        nbytes = tensor.numel() * tensor.element_size()
         if self.telemetry.should_record():
             self.telemetry.record(nbytes)
         if self.backend == "local" or tensor.numel() == 0:
             self._local(st)
-        elif self.backend == "symm" and tensor.is_cuda and tensor.dtype in (torch.float32, torch.bfloat16, torch.float16):
-            if name in self._compress_kwargs and nbytes >= self.cfg.min_compress_bytes:
-                self._compressed_symm(h, st)
-            else:
-                self._enqueue_symm(h, st, priority)
-                if flush:
-                    self.flush()
+        elif symm:
+            self._compressed_symm(h, st)
         elif self.backend == "ps":
             self._enqueue_ps(h, st, priority, version)
         else:
             self._collective(h, st, priority)
         return h
-
-    def _fast_push_pull(self, tensor, output, average, name, version, priority, flush):
-        """The native adapter's entry point; None when this call has to take the python path (compression
-        configured for the tensor, CPU / integer tensors)."""
-        nat = self._native
-        if nat is None:
-            return None
-        if self._compress_kwargs and ("byteps." + name) in self._compress_kwargs and (
-                tensor.numel() * tensor.element_size() >= self.cfg.min_compress_bytes):
-            return None
-        h = nat.try_push_pull_async(tensor, output, average, name, priority, version, flush)
-        if h < 0:
-            return None
-        if self._trace_native:
-            self._native_meta[h] = ("byteps." + name, self.core.now_us())
-        return -(h + 1)          # handles of the native adapter are negative on this side
 
     def poll(self, h: int) -> bool:
         if h < 0:
@@ -298,8 +255,6 @@ class PushPullEngine:
         st = self._handles.get(h)
         if st is None:
             return True
-        if st.pending_parts > 0:
-            return False
         if st.native >= 0:
             return self._ps.poll(st.native)
         if st.done_event is not None and not st.done_event.query():
@@ -322,8 +277,6 @@ class PushPullEngine:
         st = self._handles.get(h)
         if st is None:
             return None
-        if st.pending_parts > 0:
-            self.flush()
         if st.native >= 0:
             self._ps.wait(st.native)
         for w in st.work:
@@ -332,12 +285,7 @@ class PushPullEngine:
             if block_host:
                 st.done_event.synchronize()
             else:
-                # handles of one fused launch share their event: one wait per (event, stream) is enough
-                cur = torch.cuda.current_stream(st.output.device)
-                tag = (st.done_event, cur.cuda_stream)
-                if tag != self._last_waited:
-                    cur.wait_event(st.done_event)
-                    self._last_waited = tag
+                torch.cuda.current_stream(st.output.device).wait_event(st.done_event)
         for fn in st.post:
             fn()
         self._sample(st)
@@ -526,144 +474,11 @@ class PushPullEngine:
         return True
 
     # ------------------------------------------------------------------ symmetric-memory transport
-    def _enqueue_symm(self, h: int, st: _HandleState, priority: int):
-        t, out = st.tensor, st.output
-        self._ensure_symm(t.device)
-        es = t.element_size()
-        nbytes = t.numel() * es
-        info = self._part_cache.get(st.name)
-        if info is None or info[0] != nbytes:
-            keys = self.registry.init_tensor(st.name, nbytes, core_dtype(t.dtype), self.cfg.partition_bound(), 4096)
-            info = (nbytes, list(zip(self.registry.partitions(st.name), keys)))
-            self._part_cache[st.name] = info
-        sp, dp = t.data_ptr(), out.data_ptr()
-        self._flush_device = t.device
-        st.pending_parts = len(info[1])
-        avg, dt, dev = st.average, t.dtype, t.device
-        for (off, ln), k in info[1]:
-            self._parts.setdefault(k, []).append(_Part(k, sp + off, dp + off, ln // es, h, avg, ln, dt, dev))
-            self.queue.add(self.core.Task(k, priority, ln))
-
     def flush(self):
-        """Drain the scheduler into fused launches (deterministic on every rank
+        """Drain the native scheduler into fused launches (deterministic on every rank
         as long as ranks enqueue the same tensors between flush points)."""
         if self._native is not None:
             self._native.flush()
-        if self.queue.pending() == 0:
-            return
-        # one readiness event per flush window: everything enqueued so far was produced on this stream
-        ev = torch.cuda.Event()
-        ev.record(torch.cuda.current_stream(self._flush_device))
-        self.comm_stream.wait_event(ev)
-        batch: List[_Part] = []
-        batch_bytes = 0
-        sig = None
-        while True:
-            task = self.queue.get()
-            if task is None:
-                if batch:
-                    self._launch(batch)
-                    batch, batch_bytes, sig = [], 0, None
-                    continue   # credits were returned by _launch; try again
-                break
-            part = self._parts[task.key].pop(0)
-            psig = (part.dtype, part.average)
-            if batch and (psig != sig or batch_bytes + part.nbytes > self.cfg.group_bytes):
-                self._launch(batch)
-                batch, batch_bytes = [], 0
-            sig = psig
-            batch.append(part)
-            batch_bytes += part.nbytes
-        # all launched; nothing pending
-
-    def _wire_dtype(self, dtype: torch.dtype) -> torch.dtype:
-        w = self.cfg.wire_dtype
-        if dtype == torch.float32 and w in ("bf16", "bfloat16"):
-            return torch.bfloat16
-        if dtype == torch.float32 and w in ("fp16", "float16", "half"):
-            return torch.float16
-        return dtype
-
-    def _alloc_stage(self, nbytes: int, end_barrier: bool = True):
-        """Bump allocation over the staging ring.
-
-        A one-shot launch skips its end barrier (one NVLink round trip less): peers may still
-        be reading my window when my kernel exits.  That is safe as long as the NEXT launch uses
-        a different window - any rank that starts launch k+2 has passed launch k+1's start
-        barrier, i.e. every rank finished launch k.  If the ring wrapped onto the window of a
-        launch that had no end barrier, a barrier-only kernel fences it first."""
-        if self._native is not None:       # one allocator for both users of the staging arena
-            return self._native.alloc_stage(int(nbytes), bool(end_barrier))
-        cap = self.symm.data_bytes
-        if nbytes > cap:
-            raise RuntimeError("push_pull batch of %d bytes exceeds BYTEPS_ARENA_BYTES=%d" % (nbytes, cap))
-        if self._stage_cursor + nbytes > cap:
-            self._stage_cursor = 0
-        off = self._stage_cursor
-        self._stage_cursor = (off + nbytes + 255) // 256 * 256
-        prev = self._prev_window
-        if prev is not None and not prev[2] and off < prev[1] and prev[0] < off + nbytes:
-            self.symm.cu.barrier(self.symm.view, 1, 0, self.comm_stream.cuda_stream)
-            self.launches += 1
-        self._prev_window = (off, off + nbytes, end_barrier)
-        return off
-
-    def _seg_table(self, rows: List[List[int]], device):
-        """Upload a SegDesc table through a small pinned ring (slots are
-        recycled only after their H2D copy has completed)."""
-        n = len(rows)
-        if not self._seg_ring:
-            for _ in range(8):
-                self._seg_ring.append({"host": torch.empty((1024, 4), dtype=torch.int64).pin_memory(),
-                                       "dev": torch.empty((1024, 4), dtype=torch.int64, device=device),
-                                       "ev": None})
-        slot = self._seg_ring[self._seg_slot]
-        self._seg_slot = (self._seg_slot + 1) % len(self._seg_ring)
-        if n > slot["host"].shape[0]:
-            slot["host"] = torch.empty((n * 2, 4), dtype=torch.int64).pin_memory()
-            slot["dev"] = torch.empty((n * 2, 4), dtype=torch.int64, device=device)
-        if slot["ev"] is not None:
-            slot["ev"].synchronize()
-        slot["host"][:n] = torch.tensor(rows, dtype=torch.int64)
-        with torch.cuda.stream(self.comm_stream):
-            slot["dev"][:n].copy_(slot["host"][:n], non_blocking=True)
-            ev = torch.cuda.Event()
-            ev.record(self.comm_stream)
-        slot["ev"] = ev
-        return slot["dev"]
-
-    def _launch(self, batch: List[_Part]):
-        cu = self.symm.cu
-        dtype = batch[0].dtype
-        wire = self._wire_dtype(dtype)
-        wes = _ES[wire]
-        rows, start = [], 0
-        for p in batch:
-            rows.append([p.src, p.dst, start, p.numel])
-            start += (p.numel + 7) // 8 * 8
-        total = start
-        world = self.size
-        nbytes = total * wes
-        one_shot = nbytes <= self.cfg.one_shot_bytes and world > 1
-        end_barrier = not one_shot
-        off = self._alloc_stage(nbytes, end_barrier)
-        segs = self._seg_table(rows, batch[0].device)
-        scale = (1.0 / world) if batch[0].average else 1.0
-        threads = self.cfg.comm_threads
-        shard = nbytes if one_shot else (nbytes + world - 1) // world
-        blocks = self.cfg.comm_blocks or pick_blocks(shard, threads, 32, cap=64)
-        cu.pushpull_packed(self.symm.view, wire_code(dtype), wire_code(wire), segs.data_ptr(), len(rows), off, total,
-                           scale, blocks, threads, 0, self.symm.nvls and not one_shot, one_shot, end_barrier,
-                           self.comm_stream.cuda_stream)
-        self.launches += 1
-        ev = torch.cuda.Event()
-        ev.record(self.comm_stream)
-        for p in batch:
-            self.queue.report_finish(p.nbytes)
-            st = self._handles.get(p.handle)
-            if st is not None:
-                st.pending_parts -= 1
-                st.done_event = ev
 
     # ------------------------------------------------------------------ parameter-server transport
     _ps = None

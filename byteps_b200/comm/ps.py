@@ -362,7 +362,7 @@ class PSClient:
         cs = eng.comm_stream
         n, es = t.numel(), t.element_size()
         nbytes = (n + 7) // 8 * 8 * es
-        off = eng._alloc_stage(nbytes)
+        off = eng._native.alloc_stage(nbytes, True)
         window = ctx.tensor(off, n, t.dtype)
         ready = torch.cuda.Event()
         ready.record(torch.cuda.current_stream(dev))

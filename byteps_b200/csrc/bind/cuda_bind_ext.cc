@@ -106,46 +106,6 @@ void bind_cuda_ext(py::module_& m) {
     chk(launch_ef_correct((const void*)g, dtype, (const float*)err, ratio, (float*)corrected, n, (float*)acc, (S)s),
         "ef_correct");
   });
-  m.def("onebit_pack", [](uintptr_t corrected, size_t n, uintptr_t acc, bool use_scale, uintptr_t words,
-                          uintptr_t err_out, uintptr_t s) {
-    chk(launch_onebit_pack((const float*)corrected, n, (const float*)acc, use_scale ? 1 : 0, (uint32_t*)words,
-                           (float*)err_out, (S)s), "onebit_pack");
-  });
-  m.def("onebit_exchange_sum", [](const PeerView& pv, size_t off, size_t n, uintptr_t sum, int blocks, int channel,
-                                  uintptr_t s) {
-    chk(launch_onebit_exchange_sum(pv, off, n, (float*)sum, blocks, channel, (S)s), "onebit_exchange_sum");
-  });
-  m.def("onebit_unpack", [](uintptr_t words, size_t n, uintptr_t out, int dtype, float mult, uintptr_t s) {
-    chk(launch_onebit_unpack((const uint32_t*)words, n, (void*)out, dtype, mult, (S)s), "onebit_unpack");
-  });
-  m.def("topk_select", [](uintptr_t corrected, size_t n, uint32_t k, uintptr_t pairs, uintptr_t err_out,
-                          uintptr_t scratch, uintptr_t s) {
-    chk(launch_topk_select((const float*)corrected, n, k, (uint32_t*)pairs, (float*)err_out, (uint32_t*)scratch,
-                           (S)s), "topk_select");
-  });
-  m.def("sparse_exchange_sum", [](const PeerView& pv, size_t off, uint32_t k, size_t n, uintptr_t sum, int blocks,
-                                  int channel, uintptr_t s) {
-    chk(launch_sparse_exchange_sum(pv, off, k, n, (float*)sum, blocks, channel, (S)s), "sparse_exchange_sum");
-  });
-  m.def("sparse_add", [](uintptr_t pairs, uint32_t k, size_t n, uintptr_t sum, uintptr_t s) {
-    chk(launch_sparse_add((const uint32_t*)pairs, k, n, (float*)sum, (S)s), "sparse_add");
-  });
-  m.def("sparse_scatter", [](uintptr_t pairs, uint32_t k, size_t n, uintptr_t out, int dtype, float mult,
-                             uintptr_t s) {
-    chk(launch_sparse_scatter((const uint32_t*)pairs, k, n, (void*)out, dtype, mult, (S)s), "sparse_scatter");
-  });
-  m.def("randomk_indices", [](uintptr_t state, uint32_t k, size_t n, uintptr_t idx, uintptr_t s) {
-    chk(launch_randomk_indices((uint64_t*)state, k, n, (uint32_t*)idx, (S)s), "randomk_indices");
-  });
-  m.def("randomk_gather", [](uintptr_t corrected, uintptr_t idx, uint32_t k, size_t n, uintptr_t vals,
-                             uintptr_t err_out, uintptr_t s) {
-    chk(launch_randomk_gather((const float*)corrected, (const uint32_t*)idx, k, n, (float*)vals, (float*)err_out,
-                              (S)s), "randomk_gather");
-  });
-  m.def("dense_exchange_sum", [](const PeerView& pv, size_t off, uint32_t k, uintptr_t out, int blocks, int channel,
-                                 uintptr_t s) {
-    chk(launch_dense_exchange_sum(pv, off, k, (float*)out, blocks, channel, (S)s), "dense_exchange_sum");
-  });
   m.def("index_scatter", [](uintptr_t idx, uintptr_t vals, uint32_t k, size_t n, uintptr_t out, int dtype, float mult,
                             uintptr_t s) {
     chk(launch_index_scatter((const uint32_t*)idx, (const float*)vals, k, n, (void*)out, dtype, mult, (S)s),
@@ -156,11 +116,6 @@ void bind_cuda_ext(py::module_& m) {
                               uintptr_t err_out, uintptr_t s) {
     chk(launch_dither_quantize((const float*)corrected, n, (const float*)acc, s_levels, partition, normalize, seed,
                                step, (int8_t*)levels, (float*)scale_out, (float*)err_out, (S)s), "dither_quantize");
-  });
-  m.def("dither_exchange_sum", [](const PeerView& pv, size_t off, size_t n, int s_levels, int partition,
-                                  uintptr_t sum, int blocks, int channel, uintptr_t s) {
-    chk(launch_dither_exchange_sum(pv, off, n, s_levels, partition, (float*)sum, blocks, channel, (S)s),
-        "dither_exchange_sum");
   });
   m.def("dither_unpack", [](uintptr_t levels, uintptr_t scale, size_t n, int s_levels, int partition, uintptr_t out,
                             int dtype, float mult, uintptr_t s) {

@@ -101,200 +101,11 @@ __global__ void ef_finalize_kernel(float* acc, int nblocks) {
   }
 }
 
-// ---------------------------------------------------------------- onebit
-__global__ void onebit_pack_kernel(const float* corrected, size_t n, const float* acc, int use_scale, uint32_t* words,
-                                   float* err_out) {
-  const size_t nwords = (n + 31) / 32;
-  const float scale = use_scale ? acc[0] / (float)n : 1.0f;
-  const int lane = threadIdx.x & 31;
-  const size_t warps = ((size_t)gridDim.x * blockDim.x) >> 5;
-  for (size_t w = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < nwords; w += warps) {
-    size_t i = w * 32 + lane;
-    float v = i < n ? corrected[i] : 0.f;
-    bool neg = (i < n) && (v < 0.f);
-    uint32_t bits = __brev(__ballot_sync(0xffffffffu, neg));   // lane 0 -> MSB
-    if (lane == 0) words[w] = bits;
-    if (err_out && i < n) err_out[i] = v - (neg ? -scale : scale);
-  }
-  if (blockIdx.x == 0 && threadIdx.x == 0) reinterpret_cast<float*>(words + nwords)[0] = scale;
-}
-
-__global__ void onebit_exchange_sum_kernel(PeerView pv, size_t off, size_t n, float* sum, int channel) {
-  barrier_peers(pv, channel);
-  const size_t nwords = (n + 31) / 32;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    float acc = 0.f;
-    for (int p = 0; p < pv.world; ++p) {
-      const uint32_t* w = reinterpret_cast<const uint32_t*>(pv.data[p] + off);
-      const float scale = reinterpret_cast<const float*>(w + nwords)[0];
-      const uint32_t word = w[i >> 5];
-      acc += ((word >> (31 - (i & 31))) & 1u) ? -scale : scale;
-    }
-    sum[i] = acc;
-  }
-  barrier_peers(pv, channel);
-}
-
-template <class U>
-__global__ void onebit_unpack_kernel(const uint32_t* words, size_t n, void* out, float mult) {
-  const size_t nwords = (n + 31) / 32;
-  const float scale = reinterpret_cast<const float*>(words + nwords)[0] * mult;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    uint32_t word = words[i >> 5];
-    U::store1(out, i, ((word >> (31 - (i & 31))) & 1u) ? -scale : scale);
-  }
-}
-
-// ---------------------------------------------------------------- top-k by radix select on |x| bits
-// scratch layout (uint32): [0..255] histogram, [256] prefix, [257] mask, [258] k_remaining, [259] cnt_gt,
-// [260] cnt_eq, [261] k
-__global__ void topk_init_kernel(uint32_t* sc, uint32_t k) {
-  int t = threadIdx.x;
-  if (t < 256) sc[t] = 0;
-  if (t == 0) {
-    sc[256] = 0;
-    sc[257] = 0;
-    sc[258] = k;
-    sc[259] = 0;
-    sc[260] = 0;
-    sc[261] = k;
-  }
-}
-
-__global__ void topk_hist_kernel(const float* x, size_t n, int shift, uint32_t* sc) {
-  __shared__ uint32_t h[256];
-  for (int i = threadIdx.x; i < 256; i += blockDim.x) h[i] = 0;
-  __syncthreads();
-  const uint32_t prefix = sc[256], mask = sc[257];
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    uint32_t key = __float_as_uint(x[i]) & 0x7fffffffu;
-    if ((key & mask) == prefix) atomicAdd(&h[(key >> shift) & 0xffu], 1u);
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < 256; i += blockDim.x)
-    if (h[i]) atomicAdd(&sc[i], h[i]);
-}
-
-__global__ void topk_pick_kernel(int shift, uint32_t* sc) {
-  if (threadIdx.x == 0) {
-    uint32_t k = sc[258], cum = 0;
-    int d = 255;
-    for (; d > 0; --d) {
-      if (cum + sc[d] >= k) break;
-      cum += sc[d];
-    }
-    sc[256] |= (uint32_t)d << shift;
-    sc[257] |= 0xffu << shift;
-    sc[258] = k - cum;   // how many to take among keys sharing the new prefix
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < 256; i += blockDim.x) sc[i] = 0;
-}
-
-__global__ void topk_compact_kernel(const float* x, size_t n, uint32_t* pairs, float* err_out, uint32_t* sc) {
-  const uint32_t thr = sc[256], k_eq = sc[258], k = sc[261];
-  const uint32_t base_eq = k - k_eq;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    float v = x[i];
-    uint32_t key = __float_as_uint(v) & 0x7fffffffu;
-    bool take = false;
-    uint32_t slot = 0;
-    if (key > thr) {
-      slot = atomicAdd(&sc[259], 1u);
-      take = slot < base_eq;
-    } else if (key == thr) {
-      uint32_t e = atomicAdd(&sc[260], 1u);
-      if (e < k_eq) {
-        slot = base_eq + e;
-        take = true;
-      }
-    }
-    if (take) {
-      pairs[2 * slot] = (uint32_t)i;
-      pairs[2 * slot + 1] = __float_as_uint(v);
-    }
-    if (err_out) err_out[i] = take ? 0.f : v;
-  }
-}
-
-__global__ void sparse_exchange_sum_kernel(PeerView pv, size_t off, uint32_t k, size_t n, float* sum, int channel) {
-  barrier_peers(pv, channel);
-  const size_t total = (size_t)k * pv.world;
-  for (size_t j = blockIdx.x * (size_t)blockDim.x + threadIdx.x; j < total; j += (size_t)gridDim.x * blockDim.x) {
-    int p = (int)(j / k);
-    uint32_t r = (uint32_t)(j % k);
-    const uint32_t* pairs = reinterpret_cast<const uint32_t*>(pv.data[p] + off);
-    uint32_t idx = pairs[2 * r];
-    float val = __uint_as_float(pairs[2 * r + 1]);
-    if (idx < n) atomicAdd(&sum[idx], val);
-  }
-  barrier_peers(pv, channel);
-}
-
-// deterministic alternative to the atomic version: one launch per peer, indices are unique within a payload
-__global__ void sparse_add_kernel(const uint32_t* pairs, uint32_t k, size_t n, float* sum) {
-  for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < k; r += gridDim.x * blockDim.x) {
-    uint32_t idx = pairs[2 * r];
-    if (idx < n) sum[idx] += __uint_as_float(pairs[2 * r + 1]);
-  }
-}
-
+// ---------------------------------------------------------------- random-k: scatter of the summed values
 template <class U>
 __global__ void zero_out_kernel(void* out, size_t n) {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
     U::store1(out, i, 0.f);
-}
-
-template <class U>
-__global__ void sparse_scatter_kernel(const uint32_t* pairs, uint32_t k, size_t n, void* out, float mult) {
-  for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < k; r += gridDim.x * blockDim.x) {
-    uint32_t idx = pairs[2 * r];
-    if (idx < n) U::store1(out, idx, mult * __uint_as_float(pairs[2 * r + 1]));
-  }
-}
-
-// ---------------------------------------------------------------- random-k
-__global__ void randomk_indices_kernel(uint64_t* state, uint32_t k, uint64_t n, uint32_t* idx) {
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    uint64_t a = state[0], b = state[1];
-    for (uint32_t i = 0; i < k; ++i) {   // xorshift128+, the CPU compressor's exact stream
-      uint64_t t = a;
-      const uint64_t s = b;
-      a = s;
-      t ^= t << 23;
-      t ^= t >> 17;
-      t ^= s ^ (s >> 26);
-      b = t;
-      idx[i] = (uint32_t)((t + s) % n);
-    }
-    state[0] = a;
-    state[1] = b;
-  }
-}
-
-__global__ void copy_kernel(const float* in, float* out, size_t n) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    out[i] = in[i];
-}
-
-__global__ void randomk_gather_kernel(const float* corrected, const uint32_t* idx, uint32_t k, float* vals,
-                                      float* err_out) {
-  for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < k; r += gridDim.x * blockDim.x) {
-    vals[r] = corrected[idx[r]];
-  }
-}
-__global__ void zero_indexed_kernel(const uint32_t* idx, uint32_t k, float* err) {
-  for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < k; r += gridDim.x * blockDim.x) err[idx[r]] = 0.f;
-}
-
-__global__ void dense_exchange_sum_kernel(PeerView pv, size_t off, uint32_t k, float* out, int channel) {
-  barrier_peers(pv, channel);
-  for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < k; r += gridDim.x * blockDim.x) {
-    float acc = 0.f;
-    for (int p = 0; p < pv.world; ++p) acc += reinterpret_cast<const float*>(pv.data[p] + off)[r];
-    out[r] = acc;
-  }
-  barrier_peers(pv, channel);
 }
 
 template <class U>
@@ -366,24 +177,6 @@ __global__ void dither_quantize_kernel(const float* x, size_t n, const float* ac
   if (blockIdx.x == 0 && threadIdx.x == 0) scale_out[0] = scale;
 }
 
-__global__ void dither_exchange_sum_kernel(PeerView pv, size_t off, size_t n, int s_levels, int partition,
-                                           float* sum, int channel) {
-  barrier_peers(pv, channel);
-  const size_t lv_bytes = (n + 15) / 16 * 16;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    float acc = 0.f;
-    for (int p = 0; p < pv.world; ++p) {
-      const int8_t* lv = reinterpret_cast<const int8_t*>(pv.data[p] + off);
-      const float scale = reinterpret_cast<const float*>(pv.data[p] + off + lv_bytes)[0];
-      int q = lv[i];
-      float mag = dither_level_value(q < 0 ? -q : q, s_levels, partition) * scale;
-      acc += q < 0 ? -mag : mag;
-    }
-    sum[i] = acc;
-  }
-  barrier_peers(pv, channel);
-}
-
 template <class U>
 __global__ void dither_unpack_kernel(const int8_t* levels, const float* scale_p, size_t n, int s_levels,
                                      int partition, void* out, float mult) {
@@ -430,79 +223,6 @@ cudaError_t launch_ef_correct(const void* g, int dtype, const float* err, float 
   return cudaGetLastError();
 }
 
-cudaError_t launch_onebit_pack(const float* corrected, size_t n, const float* acc, int use_scale, uint32_t* words,
-                               float* err_out, cudaStream_t s) {
-  onebit_pack_kernel<<<grid_for(n, 1), kThreads, 0, s>>>(corrected, n, acc, use_scale, words, err_out);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_onebit_exchange_sum(const PeerView& pv, size_t off, size_t n, float* sum, int blocks, int channel,
-                                       cudaStream_t s) {
-  if (blocks < 1 || blocks > kMaxBlocks) return cudaErrorInvalidValue;
-  onebit_exchange_sum_kernel<<<blocks, kThreads, 0, s>>>(pv, off, n, sum, channel);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_onebit_unpack(const uint32_t* words, size_t n, void* out, int dtype, float mult, cudaStream_t s) {
-  DISPATCH_U(dtype, (onebit_unpack_kernel<U><<<grid_for(n), kThreads, 0, s>>>(words, n, out, mult)));
-  return cudaGetLastError();
-}
-
-cudaError_t launch_topk_select(const float* corrected, size_t n, uint32_t k, uint32_t* pairs, float* err_out,
-                               uint32_t* scratch, cudaStream_t s) {
-  if (k == 0 || k > n) return cudaErrorInvalidValue;
-  topk_init_kernel<<<1, 256, 0, s>>>(scratch, k);
-  for (int shift = 24; shift >= 0; shift -= 8) {
-    topk_hist_kernel<<<grid_for(n), kThreads, 0, s>>>(corrected, n, shift, scratch);
-    topk_pick_kernel<<<1, 256, 0, s>>>(shift, scratch);
-  }
-  topk_compact_kernel<<<grid_for(n), kThreads, 0, s>>>(corrected, n, pairs, err_out, scratch);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_sparse_exchange_sum(const PeerView& pv, size_t off, uint32_t k, size_t n, float* sum, int blocks,
-                                       int channel, cudaStream_t s) {
-  if (blocks < 1 || blocks > kMaxBlocks) return cudaErrorInvalidValue;
-  cudaError_t e = cudaMemsetAsync(sum, 0, n * sizeof(float), s);
-  if (e != cudaSuccess) return e;
-  sparse_exchange_sum_kernel<<<blocks, kThreads, 0, s>>>(pv, off, k, n, sum, channel);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_sparse_add(const uint32_t* pairs, uint32_t k, size_t n, float* sum, cudaStream_t s) {
-  sparse_add_kernel<<<grid_for(k, 1), kThreads, 0, s>>>(pairs, k, n, sum);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_sparse_scatter(const uint32_t* pairs, uint32_t k, size_t n, void* out, int dtype, float mult,
-                                  cudaStream_t s) {
-  DISPATCH_U(dtype, (zero_out_kernel<U><<<grid_for(n), kThreads, 0, s>>>(out, n)));
-  DISPATCH_U(dtype, (sparse_scatter_kernel<U><<<grid_for(k, 1), kThreads, 0, s>>>(pairs, k, n, out, mult)));
-  return cudaGetLastError();
-}
-
-cudaError_t launch_randomk_indices(uint64_t* state, uint32_t k, size_t n, uint32_t* idx, cudaStream_t s) {
-  randomk_indices_kernel<<<1, 32, 0, s>>>(state, k, (uint64_t)n, idx);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_randomk_gather(const float* corrected, const uint32_t* idx, uint32_t k, size_t n, float* vals,
-                                  float* err_out, cudaStream_t s) {
-  randomk_gather_kernel<<<grid_for(k, 1), kThreads, 0, s>>>(corrected, idx, k, vals, err_out);
-  if (err_out) {
-    if (err_out != corrected) copy_kernel<<<grid_for(n), kThreads, 0, s>>>(corrected, err_out, n);
-    zero_indexed_kernel<<<grid_for(k, 1), kThreads, 0, s>>>(idx, k, err_out);
-  }
-  return cudaGetLastError();
-}
-
-cudaError_t launch_dense_exchange_sum(const PeerView& pv, size_t off, uint32_t k, float* vals_sum, int blocks,
-                                      int channel, cudaStream_t s) {
-  if (blocks < 1 || blocks > kMaxBlocks) return cudaErrorInvalidValue;
-  dense_exchange_sum_kernel<<<blocks, kThreads, 0, s>>>(pv, off, k, vals_sum, channel);
-  return cudaGetLastError();
-}
-
 cudaError_t launch_index_scatter(const uint32_t* idx, const float* vals, uint32_t k, size_t n, void* out, int dtype,
                                  float mult, cudaStream_t s) {
   DISPATCH_U(dtype, (zero_out_kernel<U><<<grid_for(n), kThreads, 0, s>>>(out, n)));
@@ -516,13 +236,6 @@ cudaError_t launch_dither_quantize(const float* corrected, size_t n, const float
   if (s_levels < 1 || s_levels > 126) return cudaErrorInvalidValue;
   dither_quantize_kernel<<<grid_for(n), kThreads, 0, s>>>(corrected, n, acc, s_levels, partition, normalize, seed,
                                                          step, levels, scale_out, err_out);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_dither_exchange_sum(const PeerView& pv, size_t off, size_t n, int s_levels, int partition,
-                                       float* sum, int blocks, int channel, cudaStream_t s) {
-  if (blocks < 1 || blocks > kMaxBlocks) return cudaErrorInvalidValue;
-  dither_exchange_sum_kernel<<<blocks, kThreads, 0, s>>>(pv, off, n, s_levels, partition, sum, channel);
   return cudaGetLastError();
 }
 

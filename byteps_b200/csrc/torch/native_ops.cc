@@ -168,10 +168,10 @@ class NativeSymmOps {
     return h;
   }
 
-  // Fast path used by the python engine: takes the user's name (the "byteps." prefix is added here),
+  // Entry point of the python engine: takes the user's name (the "byteps." prefix is added here),
   // returns -1 instead of raising when the tensors are not something this adapter moves (CPU tensors,
-  // integer dtypes, empty tensors) so the caller can fall back.  eager: launch right away when the tensor is
-  // at least one partition long (it overlaps with whatever the caller enqueues next).
+  // integer dtypes, empty tensors, an output of another dtype or size).  eager: launch right away when the
+  // tensor is at least one partition long (it overlaps with whatever the caller enqueues next).
   int try_push_pull_async(const at::Tensor& t, const at::Tensor& out, bool average, const std::string& name,
                           int priority, int version, bool eager) {
     if (!t.is_cuda() || !out.is_cuda() || t.numel() == 0 || wire_of(t.scalar_type()) < 0 ||
@@ -243,8 +243,7 @@ class NativeSymmOps {
   }
   size_t launches() const { return launches_; }
 
-  // Staging windows are bump-allocated; the python engine (CPU-server hierarchical path) shares
-  // the allocator through this call.  See comm/engine.py::_alloc_stage for the reuse rule.
+  // The CPU-server hierarchical path (comm/ps.py) stages its windows through the same allocator.
   size_t alloc_stage(size_t nbytes, bool end_barrier) {
     std::lock_guard<std::mutex> g(mu_);
     return alloc_stage_locked(nbytes, end_barrier);
@@ -281,12 +280,16 @@ class NativeSymmOps {
     return e;
   }
 
+  // Bump allocation over the staging ring.  A one-shot launch skips its end barrier (one NVLink
+  // round trip less): peers may still be reading my window when my kernel exits.  That is safe as
+  // long as the NEXT launch uses a different window - any rank that starts launch k+2 has passed
+  // launch k+1's start barrier, i.e. every rank finished launch k.  If the ring wrapped onto the
+  // window of a launch that had no end barrier, a barrier-only kernel fences it first.
   size_t alloc_stage_locked(size_t nbytes, bool end_barrier) {
     if (nbytes > arena_bytes_) throw std::runtime_error("push_pull batch exceeds BYTEPS_ARENA_BYTES");
     if (stage_cursor_ + nbytes > arena_bytes_) stage_cursor_ = 0;
     const size_t off = stage_cursor_;
     stage_cursor_ = (off + nbytes + 255) / 256 * 256;
-    // a one-shot launch has no end barrier: its window may only be reused behind a barrier
     if (have_prev_ && !prev_end_barrier_ && off < prev_hi_ && prev_lo_ < off + nbytes) {
       cuda_check(launch_barrier(pv_, 1, 0, comm_), "barrier");
       ++launches_;

@@ -15,7 +15,7 @@ lr ratio, nesterov momentum.  Pipeline for one tensor, all on one stream:
               sweep, then one pass that writes the user's tensor (x 1/size when averaging)
 
 (csrc/kernels/compress_fused.cu; dithering quantises with the kernels of compress.cu and uses the same
-push + local-sum exchange.)
+push + local-sum exchange, and random-k scatters its sums with compress.cu's index_scatter.)
 
 The second stage reproduces the reference's server-side compression
 (server.cc:92-118) so results follow the same two-stage contract its tests

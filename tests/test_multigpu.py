@@ -23,6 +23,20 @@ def _pushpull(rank, world):
             ref = ((torch.arange(n, device="cuda") % 13).float() * tot).to(dt)
             assert torch.equal(x, x0)
             assert torch.allclose(y.float(), ref.float(), rtol=1e-2 if dt != torch.float32 else 1e-6), (dt, n)
+    # unnamed tensors (auto-named per call) go through the same native adapter
+    launches0 = engine()._native.launches
+    for dt in (torch.float32, torch.bfloat16):
+        for n in (4096, 8_000_000):
+            x = (torch.arange(n, device="cuda") % 13).to(dt) * (rank + 1)
+            x0 = x.clone()
+            y = bps.synchronize(bps.push_pull_async(x, average=False))
+            tot = sum(r + 1 for r in range(world))
+            ref = ((torch.arange(n, device="cuda") % 13).float() * tot).to(dt)
+            assert torch.equal(x, x0)
+            assert torch.allclose(y.float(), ref.float(), rtol=1e-2 if dt != torch.float32 else 1e-6), (dt, n)
+    assert engine()._native.launches > launches0 and engine().outstanding() == 0
+    with pytest.raises(ValueError):           # the kernels write input-dtype elements through the output pointer
+        engine().push_pull_async(x, torch.empty(n, device="cuda", dtype=torch.float16), False, "mismatch")
     # many small tensors issued back to back, synchronised at the end (priority order inside the flush)
     ts = [torch.full((1000 + i,), float(rank), device="cuda") for i in range(20)]
     hs = [bps.push_pull_async_inplace(t, average=True, name="many%d" % i, priority=-i) for i, t in enumerate(ts)]
