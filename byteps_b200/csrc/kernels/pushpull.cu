@@ -367,11 +367,13 @@ cudaError_t launch_pushpull_fused_opt(const PeerView& pv, int grad_dtype, int wi
     return cudaErrorInvalidValue;                                                                                    \
   }                                                                                                                  \
   return cudaGetLastError();
+  // exactly the (gradient, wire) pairs the bucket layer produces: fp32 gradients on an fp32, bf16 or fp16 wire,
+  // 16-bit gradients on their own dtype; parameters always have the gradient dtype
   if (grad_dtype == WIRE_BF16 && wire == WIRE_BF16 && param_dtype == WIRE_BF16) { BPS_FUSED(TagBF16, TagBF16, TagBF16) }
   if (grad_dtype == WIRE_F32 && wire == WIRE_F32 && param_dtype == WIRE_F32) { BPS_FUSED(TagF32, TagF32, TagF32) }
   if (grad_dtype == WIRE_F32 && wire == WIRE_BF16 && param_dtype == WIRE_F32) { BPS_FUSED(TagF32, TagBF16, TagF32) }
+  if (grad_dtype == WIRE_F32 && wire == WIRE_F16 && param_dtype == WIRE_F32) { BPS_FUSED(TagF32, TagF16, TagF32) }
   if (grad_dtype == WIRE_F16 && wire == WIRE_F16 && param_dtype == WIRE_F16) { BPS_FUSED(TagF16, TagF16, TagF16) }
-  if (grad_dtype == WIRE_BF16 && wire == WIRE_F32 && param_dtype == WIRE_BF16) { BPS_FUSED(TagBF16, TagF32, TagBF16) }
 #undef BPS_FUSED
   return cudaErrorInvalidValue;
 }

@@ -1,13 +1,13 @@
-"""Numerics of the sm_90a push-pull kernels against plain PyTorch fp32 references.
+"""Numerics of the sm_90a push-pull kernels against plain PyTorch fp32 references, and of the fused
+optimizer kernels against torch.optim in float64.
 
 Multi-peer behaviour is exercised on ONE GPU with `VirtualCluster`: N virtual
 ranks, N concurrent kernels on N streams, same flag protocol and peer-pointer
 arithmetic as the real multi-process setup.
 """
-import struct
-
 import pytest
 import torch
+from _fused_opt import ENGINE_DTYPES, check_fused_optimizer, dt_id, fused_cases
 
 pytestmark = pytest.mark.gpu
 
@@ -164,76 +164,15 @@ def test_packed_pushpull_virtual(world, one_shot, user, wire):
             assert torch.isfinite(a.float()).all()
 
 
-def _hp(lr=0.1, wd=0.0, mom=0.0, damp=0.0, b1=0.9, b2=0.999, eps=1e-8, t=1, nesterov=0, adamw=0, first=1, gs=1.0):
-    return struct.pack("<9f3if3i", lr, wd, mom, damp, b1, b2, eps, 1 - b1 ** t, 1 - b2 ** t, nesterov, adamw, first,
-                       gs, 0, 0, 0)
+_FUSED_CASES = [(w, eng, d, o) for eng in ("lsu", "pack", "tma") for w, d, o in fused_cases(ENGINE_DTYPES[eng])]
 
 
-@pytest.mark.parametrize("world", [1, 4])
-@pytest.mark.parametrize("kind", ["sgd", "sgd_nesterov", "adam", "adamw"])
-@pytest.mark.parametrize("dt", ["f32", "bf16"])
-@pytest.mark.parametrize("engine", ["lsu", "tma"])
-def test_fused_optimizer_virtual(world, kind, dt, engine):
-    """grad window + param window in the arena; master/momentum shards local.  engine = register
-    (LSU) kernel or the TMA-streamed one (state through a shared-memory ring of bulk copies)."""
-    from byteps_b200.comm.symm import VirtualCluster
-
-    cu = _cu()
-    dtype = DT[dt]
-    n = 8 * 777 if engine == "lsu" else 8 * 5003     # several tiles per CTA + a ragged last tile
-    es = torch.empty((), dtype=dtype).element_size()
-    goff, poff = 0, (n * es + 255) // 256 * 256
-    vc = VirtualCluster(world, "cuda:0", 1 << 21)
-    torch.manual_seed(2)
-    w0 = torch.randn(n, device="cuda").to(dtype)
-    ref_w = torch.nn.Parameter(w0.float().clone())
-    if kind.startswith("sgd"):
-        ref_opt = torch.optim.SGD([ref_w], lr=0.1, momentum=0.9, weight_decay=0.01, nesterov=kind.endswith("nesterov"))
-    elif kind == "adam":
-        ref_opt = torch.optim.Adam([ref_w], lr=0.01, weight_decay=0.01)
-    else:
-        ref_opt = torch.optim.AdamW([ref_w], lr=0.01, weight_decay=0.01)
-    masters, s0s, s1s = [], [], []
-    for r in range(world):
-        b, e = cu.shard_units(n // 8, world, r)
-        m = torch.zeros(max((e - b) * 8, 8), device="cuda")
-        m[:(e - b) * 8] = w0.float()[b * 8:e * 8]
-        masters.append(m)
-        s0s.append(torch.zeros_like(m))
-        s1s.append(torch.zeros_like(m))
-        vc.arenas[r][poff:poff + n * es].view(dtype).copy_(w0)
-    hp_dev = torch.zeros(64, dtype=torch.uint8, device="cuda")
-    for step in range(1, 4):
-        grads = [torch.randn(n, device="cuda").to(dtype) for _ in range(world)]
-        for r in range(world):
-            vc.arenas[r][goff:goff + n * es].view(dtype).copy_(grads[r])
-        if kind.startswith("sgd"):
-            blob = _hp(lr=0.1, wd=0.01, mom=0.9, nesterov=int(kind.endswith("nesterov")), first=int(step == 1))
-            code = cu.OPT_SGD
-        else:
-            blob = _hp(lr=0.01, wd=0.01, t=step, adamw=int(kind == "adamw"), first=int(step == 1))
-            code = cu.OPT_ADAM
-        cu.write_blob(hp_dev.data_ptr(), blob, torch.cuda.current_stream().cuda_stream)
-        if engine == "lsu":
-            vc.run(lambda r, view, arena, s: cu.pushpull_fused_opt(
-                view, _code(dtype), _code(dtype), _code(dtype), code, 0, 0, goff, poff, n, 1.0 / world,
-                masters[r].data_ptr(), s0s[r].data_ptr(), s1s[r].data_ptr(), hp_dev.data_ptr(), 2, 256, 0, False, s))
-        else:
-            vc.run(lambda r, view, arena, s: cu.pushpull_fused_opt_tma(
-                view, _code(dtype), code, goff, poff, n, 1.0 / world, masters[r].data_ptr(), s0s[r].data_ptr(),
-                s1s[r].data_ptr(), hp_dev.data_ptr(), 2, 3, False, 0, s))
-        torch.cuda.synchronize()
-        g = torch.stack([x.float() for x in grads]).sum(0) / world
-        ref_w.grad = g
-        ref_opt.step()
-        for r in range(world):
-            got = vc.arenas[r][poff:poff + n * es].view(dtype).float()
-            tol = 1e-5 if dtype == torch.float32 else 1.2e-2
-            assert torch.allclose(got, ref_w.detach(), atol=tol, rtol=tol), (step, r, (got - ref_w.detach()).abs().max())
-    # fp32 masters track the reference much more tightly than the bf16 copies
-    full = torch.cat([masters[r][:(cu.shard_units(n // 8, world, r)[1] - cu.shard_units(n // 8, world, r)[0]) * 8]
-                      for r in range(world)])
-    assert torch.allclose(full, ref_w.detach(), atol=2e-2 if dtype != torch.float32 else 1e-5)
+@pytest.mark.parametrize("world,engine,dtypes,opt", _FUSED_CASES,
+                         ids=["%s-%s-%s-%d" % (e, dt_id(d), o, w) for w, e, d, o in _FUSED_CASES])
+def test_fused_optimizer_virtual(world, engine, dtypes, opt):
+    """Register (LSU) kernel with gradients in the arena or packed from user tensors through a wire cast, and the
+    TMA-streamed kernel: against torch.optim in float64 (see _fused_opt.check_fused_optimizer)."""
+    check_fused_optimizer(world, engine, dtypes[0], dtypes[1], opt)
 
 
 def test_reduce_scatter_then_all_gather_virtual():

@@ -2,11 +2,11 @@
 numerics against fp32 PyTorch references, bit-identical replicas, producer marks, CUDA-graph
 replays, and the scheduling contract of the reference's BytePSScheduledQueue
 (/root/reference/byteps/common/scheduled_queue.cc:82-163): priority desc, key asc, byte credits.
+Fused-optimizer descriptors are checked against torch.optim in float64 (tests/_fused_opt.py).
 """
-import struct
-
 import pytest
 import torch
+from _fused_opt import ENGINE_DTYPES, check_fused_optimizer, dt_id, fused_cases
 
 pytestmark = pytest.mark.gpu
 
@@ -23,11 +23,6 @@ def _code(dt):
     from byteps_b200.comm.symm import wire_code
 
     return wire_code(dt)
-
-
-def _hp(lr=0.1, wd=0.0, mom=0.0, damp=0.0, b1=0.9, b2=0.999, eps=1e-8, t=1, nesterov=0, adamw=0, first=1, gs=1.0):
-    return struct.pack("<9f3if3i", lr, wd, mom, damp, b1, b2, eps, 1 - b1 ** t, 1 - b2 ** t, nesterov, adamw, first,
-                       gs, 0, 0, 0)
 
 
 def _layout(sizes, es):
@@ -89,68 +84,14 @@ def test_ring_allreduce_virtual(world, dt, self_mark):
             assert torch.allclose(outs[0].float(), ref, atol=tol * max(1.0, ref.abs().max().item()), rtol=tol), (it, i)
 
 
-@pytest.mark.parametrize("world", [1, 4])
-@pytest.mark.parametrize("kind", ["sgd", "adamw"])
-@pytest.mark.parametrize("dt", ["f32", "bf16"])
-def test_ring_fused_optimizer_virtual(world, kind, dt):
-    """Fused optimizer descriptors: 3 buckets, 3 steps, against torch.optim on the mean gradient."""
-    from byteps_b200.comm.symm import VirtualCluster
-    from byteps_b200.ops.ring import RingEntry, RingTable
+_RING_FUSED_CASES = fused_cases(ENGINE_DTYPES["ring"])
 
-    cu = _cu()
-    dtype = DT[dt]
-    es = torch.empty((), dtype=dtype).element_size()
-    sizes = [8 * 777, 8 * 5003, 8 * 11]
-    goffs, mid = _layout(sizes, es)
-    poffs = [mid + o for o in goffs]
-    vc = VirtualCluster(world, "cuda:0", 2 * mid + 4096)
-    torch.manual_seed(2)
-    w0 = [torch.randn(n, device="cuda").to(dtype) for n in sizes]
-    ref_w = [torch.nn.Parameter(w.float().clone()) for w in w0]
-    if kind == "sgd":
-        ref_opt = torch.optim.SGD(ref_w, lr=0.1, momentum=0.9, weight_decay=0.01)
-        code, rkind = cu.OPT_SGD, cu.RING_SGD
-    else:
-        ref_opt = torch.optim.AdamW(ref_w, lr=0.01, weight_decay=0.01)
-        code, rkind = cu.OPT_ADAM, cu.RING_ADAM
-    del code
-    hp_dev = torch.zeros(64, dtype=torch.uint8, device="cuda")
-    state = []   # [rank][bucket] -> (master, s0, s1)
-    tables = []
-    for r in range(world):
-        st, entries = [], []
-        for i, n in enumerate(sizes):
-            b, e = cu.shard_units(n // 8, world, r)
-            m = torch.zeros(max((e - b) * 8, 8), device="cuda")
-            m[:(e - b) * 8] = w0[i].float()[b * 8:e * 8]
-            st.append((m, torch.zeros_like(m), torch.zeros_like(m)))
-            vc.arenas[r][poffs[i]:poffs[i] + n * es].view(dtype).copy_(w0[i])
-            entries.append(RingEntry(grad_off=goffs[i], param_off=poffs[i], numel=n, wire=_code(dtype), slot=i,
-                                     kind=rkind, scale=1.0 / world, master=m.data_ptr(), state0=st[-1][1].data_ptr(),
-                                     state1=st[-1][2].data_ptr(), hp=hp_dev.data_ptr()))
-        state.append(st)
-        tables.append(RingTable(entries, "cuda:0"))
-    for step in range(1, 4):
-        grads = [[torch.randn(n, device="cuda").to(dtype) for n in sizes] for _ in range(world)]
-        for r in range(world):
-            for i, n in enumerate(sizes):
-                vc.arenas[r][goffs[i]:goffs[i] + n * es].view(dtype).copy_(grads[r][i])
-        if kind == "sgd":
-            blob = _hp(lr=0.1, wd=0.01, mom=0.9, first=int(step == 1))
-        else:
-            blob = _hp(lr=0.01, wd=0.01, t=step, adamw=1, first=int(step == 1))
-        cu.write_blob(hp_dev.data_ptr(), blob, torch.cuda.current_stream().cuda_stream)
-        vc.run(lambda r, view, arena, s: tables[r].launch(view, 3, s))
-        torch.cuda.synchronize()
-        for i in range(len(sizes)):
-            ref_w[i].grad = torch.stack([grads[r][i].float() for r in range(world)]).sum(0) / world
-        ref_opt.step()
-        for r in range(world):
-            for i, n in enumerate(sizes):
-                got = vc.arenas[r][poffs[i]:poffs[i] + n * es].view(dtype)
-                assert torch.equal(got, vc.arenas[0][poffs[i]:poffs[i] + n * es].view(dtype))
-                tol = 1e-5 if dtype == torch.float32 else 1.2e-2
-                assert torch.allclose(got.float(), ref_w[i].detach(), atol=tol, rtol=tol), (step, r, i)
+
+@pytest.mark.parametrize("world,dtypes,opt", _RING_FUSED_CASES,
+                         ids=["%s-%s-%d" % (dt_id(d), o, w) for w, d, o in _RING_FUSED_CASES])
+def test_ring_fused_optimizer_virtual(world, dtypes, opt):
+    """RING_SGD / RING_ADAM descriptors: three buckets in one table, against torch.optim in float64."""
+    check_fused_optimizer(world, "ring", dtypes[0], dtypes[1], opt)
 
 
 def _sched_order(credit_bytes, sched=True, world=4):
