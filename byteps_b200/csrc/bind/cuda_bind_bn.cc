@@ -1,0 +1,58 @@
+// pybind11 surface of the fused batch-norm / residual / ReLU kernels (kernels/bn_act.cu).
+#include <cuda_runtime_api.h>
+#include <pybind11/pybind11.h>
+
+#include <stdexcept>
+#include <string>
+
+#include "bind/cuda_bind_ext.h"
+#include "kernels/bn_act.cuh"
+
+namespace py = pybind11;
+using namespace bps;
+
+namespace {
+void chk(cudaError_t e, const char* what) {
+  if (e != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(e));
+}
+}  // namespace
+
+void bind_cuda_bn(py::module_& m) {
+  m.def("bn_act_workspace", [](size_t M, int C) {
+    return py::make_tuple(bn_act_workspace_floats(M, C), bn_act_counters(C));
+  }, "(fp32 workspace floats, uint32 counters) of one bn_act_fwd_stats / bn_act_bwd_reduce launch");
+
+  m.def("bn_act_fwd_stats", [](uintptr_t x, int dtype, size_t M, int C, float eps, float momentum,
+                               uintptr_t running_mean, uintptr_t running_var, uintptr_t save_mean,
+                               uintptr_t save_invstd, uintptr_t ws, uintptr_t counters, uintptr_t s) {
+    chk(launch_bn_act_fwd_stats((const void*)x, dtype, M, C, eps, momentum, (float*)running_mean, (float*)running_var,
+                                (float*)save_mean, (float*)save_invstd, (float*)ws, (uint32_t*)counters,
+                                (cudaStream_t)s),
+        "bn_act_fwd_stats");
+  });
+  m.def("bn_act_fwd_apply", [](uintptr_t x, uintptr_t residual, int dtype, size_t M, int C, uintptr_t mean,
+                               uintptr_t invstd, uintptr_t weight, uintptr_t bias, bool relu, uintptr_t y,
+                               uintptr_t mask, uintptr_t s) {
+    chk(launch_bn_act_fwd_apply((const void*)x, (const void*)residual, dtype, M, C, (const float*)mean,
+                                (const float*)invstd, (const float*)weight, (const float*)bias, relu ? 1 : 0,
+                                (void*)y, (uint8_t*)mask, (cudaStream_t)s),
+        "bn_act_fwd_apply");
+  });
+  m.def("bn_act_bwd_reduce", [](uintptr_t dy, uintptr_t x, uintptr_t mask, int dtype, size_t M, int C, uintptr_t mean,
+                                uintptr_t invstd, uintptr_t dweight, uintptr_t dbias, uintptr_t ws, uintptr_t counters,
+                                uintptr_t s) {
+    chk(launch_bn_act_bwd_reduce((const void*)dy, (const void*)x, (const uint8_t*)mask, dtype, M, C,
+                                 (const float*)mean, (const float*)invstd, (float*)dweight, (float*)dbias, (float*)ws,
+                                 (uint32_t*)counters, (cudaStream_t)s),
+        "bn_act_bwd_reduce");
+  });
+  m.def("bn_act_bwd_apply", [](uintptr_t dy, uintptr_t x, uintptr_t mask, int dtype, size_t M, int C, uintptr_t mean,
+                               uintptr_t invstd, uintptr_t weight, uintptr_t dweight, uintptr_t dbias, uintptr_t dx,
+                               uintptr_t dresidual, uintptr_t s) {
+    chk(launch_bn_act_bwd_apply((const void*)dy, (const void*)x, (const uint8_t*)mask, dtype, M, C,
+                                (const float*)mean, (const float*)invstd, (const float*)weight,
+                                (const float*)dweight, (const float*)dbias, (void*)dx, (void*)dresidual,
+                                (cudaStream_t)s),
+        "bn_act_bwd_apply");
+  });
+}

@@ -1,0 +1,542 @@
+// Fused NHWC batch norm + residual add + ReLU (see bn_act.cuh).
+//
+// All four passes share one thread layout.  A thread owns a "unit": 8 consecutive channels of a row, i.e. one
+// 16-byte vector for 16-bit activations (two for fp32) and one mask byte.  A block of kT threads covers CB units
+// of one channel group (CB a power of two <= 32; blockIdx.y selects the group) times RL = kT / CB rows, and
+// blockIdx.x walks the rows.  A thread therefore keeps the same channels for the whole launch: their parameters
+// live in registers, and a warp touches 512 contiguous bytes of a 16-bit row when C >= 256.
+#include "kernels/bn_act.cuh"
+
+#include "kernels/common.cuh"
+#include "kernels/pushpull.cuh"
+
+namespace bps {
+
+namespace {
+
+constexpr int kT = 256;
+constexpr int kCh = 8;                  // channels per unit
+constexpr int kMaxCB = 32;              // units per block row of an elementwise pass
+// Units per block row of a reduction pass.  Narrow channel groups leave few chunk partials per channel, and the
+// finalize gives each channel kT / (CB * kCh) threads, so its sums stay short.  8 units are a full 128-byte line
+// of a 16-bit row, which no two blocks then share; that pays once C >= 256 leaves at least 4 groups.  Narrower C
+// keeps 4-unit groups: with 1 or 2 groups the finalize's per-thread sums would be too long.
+int red_cb(int C) { return C >= 256 ? 8 : 4; }
+// Every pass is sized to one full wave: kBlocksPerSM resident blocks on every SM (the register budget
+// __launch_bounds__ enforces), each walking its rows with 16-byte loads of several rows in flight.  A second,
+// partial wave would leave most SMs idle for its whole duration.
+constexpr int kBlocksPerSM = 3;
+constexpr int kBwdApplyBlocksPerSM = 2;   // its per-channel coefficients and two rows in flight need ~90 registers
+constexpr int kMinRows = 4;             // fewest rows a thread of a reduction pass walks
+
+struct Geo {
+  int shift;   // log2(CB)
+  int ncb;     // channel groups (gridDim.y)
+  int rl;      // rows per block step (RL)
+};
+
+Geo geo(int C, int max_cb) {
+  const int units = C / kCh;
+  int shift = 0;
+  while ((2 << shift) <= units && (2 << shift) <= max_cb) ++shift;
+  return Geo{shift, (units + (1 << shift) - 1) >> shift, kT >> shift};
+}
+
+// Rows per chunk of a reduction pass (a multiple of RL) and the chunk count (gridDim.x).
+int wave_blocks(int per_sm = kBlocksPerSM) {
+  int dev = 0, sms = 132;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    sms = 132;
+  return sms * per_sm;
+}
+
+void chunks(size_t M, const Geo& g, size_t* rpc, int* nchunks) {
+  const size_t want = (size_t)(wave_blocks() / g.ncb > 0 ? wave_blocks() / g.ncb : 1);
+  size_t r = (M + want - 1) / want;
+  if (r < (size_t)g.rl * kMinRows) r = (size_t)g.rl * kMinRows;
+  r = (r + g.rl - 1) / g.rl * g.rl;
+  *rpc = r;
+  *nchunks = (int)((M + r - 1) / r);
+}
+
+template <class U>
+struct Unit {
+  static constexpr int kVecs = kCh / U::kPerVec;
+  __device__ static __forceinline__ void load(const void* base, size_t unit, float* f) {
+    const Vec16* p = reinterpret_cast<const Vec16*>(base) + unit * kVecs;
+#pragma unroll
+    for (int v = 0; v < kVecs; ++v) U::unpack(ld_stream16(p + v), f + v * U::kPerVec);
+  }
+  __device__ static __forceinline__ void store(void* base, size_t unit, const float* f) {
+    Vec16* p = reinterpret_cast<Vec16*>(base) + unit * kVecs;
+#pragma unroll
+    for (int v = 0; v < kVecs; ++v) st_stream16(p + v, U::pack(f + v * U::kPerVec));
+  }
+};
+
+__device__ __forceinline__ void welford_push(float& n, float* mean, float* m2, const float* f) {
+  n += 1.f;
+  const float inv = __frcp_rn(n);
+#pragma unroll
+  for (int k = 0; k < kCh; ++k) {
+    const float d = f[k] - mean[k];
+    mean[k] = fmaf(d, inv, mean[k]);
+    m2[k] = fmaf(d, f[k] - mean[k], m2[k]);
+  }
+}
+
+// Chan's merge of (nb, mean_b, m2_b) into (n, mean, m2); the count is shared by the K channels.
+template <int K>
+__device__ __forceinline__ void chan_merge(float& n, float* mean, float* m2, float nb, const float* mb,
+                                           const float* m2b) {
+  if (nb == 0.f) return;
+  if (n == 0.f) {
+    n = nb;
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+      mean[k] = mb[k];
+      m2[k] = m2b[k];
+    }
+    return;
+  }
+  const float nn = n + nb, fb = nb / nn, w = n * fb;
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    const float d = mb[k] - mean[k];
+    mean[k] = fmaf(d, fb, mean[k]);
+    m2[k] = m2[k] + m2b[k] + d * d * w;
+  }
+  n = nn;
+}
+
+// Fixed-order tree over the `lanes` threads of a column: thread t = lane * cols + col (t == threadIdx.x);
+// the result is in lane 0.
+template <int K>
+__device__ __forceinline__ void tree_welford(float& n, float* mean, float* m2, int lane, int cols, int lanes) {
+  __shared__ float sh[2 * K + 1][kT];
+  const int t = threadIdx.x;
+  for (int s = lanes >> 1; s >= 1; s >>= 1) {
+    __syncthreads();
+    if (lane >= s && lane < 2 * s) {
+      sh[0][t] = n;
+#pragma unroll
+      for (int k = 0; k < K; ++k) {
+        sh[1 + k][t] = mean[k];
+        sh[1 + K + k][t] = m2[k];
+      }
+    }
+    __syncthreads();
+    if (lane < s) {
+      const int p = t + s * cols;
+      float mb[K], m2b[K];
+#pragma unroll
+      for (int k = 0; k < K; ++k) {
+        mb[k] = sh[1 + k][p];
+        m2b[k] = sh[1 + K + k][p];
+      }
+      chan_merge<K>(n, mean, m2, sh[0][p], mb, m2b);
+    }
+  }
+}
+
+template <int K>
+__device__ __forceinline__ void tree_sum2(float* a, float* b, int lane, int cols, int lanes) {
+  __shared__ float sh[2 * K][kT];
+  const int t = threadIdx.x;
+  for (int s = lanes >> 1; s >= 1; s >>= 1) {
+    __syncthreads();
+    if (lane >= s && lane < 2 * s) {
+#pragma unroll
+      for (int k = 0; k < K; ++k) {
+        sh[k][t] = a[k];
+        sh[K + k][t] = b[k];
+      }
+    }
+    __syncthreads();
+    if (lane < s) {
+      const int p = t + s * cols;
+#pragma unroll
+      for (int k = 0; k < K; ++k) {
+        a[k] += sh[k][p];
+        b[k] += sh[K + k][p];
+      }
+    }
+  }
+}
+
+// Finalize layout of the last block of a channel group: nc = CB * kCh channels, tpc = kT / nc threads per channel
+// (thread t: channel t % nc, lane t / nc).  Each lane sums a fixed stride of the G chunk partials, then a fixed
+// tree adds the lanes; every lane of the channel gets the result.
+struct Fin {
+  int nc, tpc, cl, sub;
+  __device__ Fin(int CB) : nc(CB * kCh), tpc(kT / (CB * kCh)), cl(threadIdx.x % (CB * kCh)),
+                           sub(threadIdx.x / (CB * kCh)) {}
+  __device__ float all_sum(float v) const {
+    __shared__ float out[kT];
+    float dummy = 0.f;
+    tree_sum2<1>(&v, &dummy, sub, nc, tpc);
+    __syncthreads();
+    if (sub == 0) out[cl] = v;
+    __syncthreads();
+    return out[cl];
+  }
+};
+
+template <class U>
+__global__ void __launch_bounds__(kT, kBlocksPerSM) bn_act_fwd_stats_kernel(const void* __restrict__ x, size_t M, int C, int shift,
+                                                             size_t rpc, float eps, float momentum, float* run_mean,
+                                                             float* run_var, float* save_mean, float* save_invstd,
+                                                             float* ws, uint32_t* counters) {
+  const int units = C / kCh, CB = 1 << shift, RL = kT >> shift;
+  const int col = threadIdx.x & (CB - 1), lane = threadIdx.x >> shift;
+  const int u = blockIdx.y * CB + col;
+  const size_t r0 = (size_t)blockIdx.x * rpc, r1 = min(M, r0 + rpc);
+  float n = 0.f, mean[kCh], m2[kCh];
+#pragma unroll
+  for (int k = 0; k < kCh; ++k) mean[k] = m2[k] = 0.f;
+  if (u < units) {
+    size_t r = r0 + lane;
+    for (; r + 3 * RL < r1; r += 4 * RL) {
+      float f[4][kCh];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) Unit<U>::load(x, (r + j * RL) * units + u, f[j]);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) welford_push(n, mean, m2, f[j]);
+    }
+    for (; r < r1; r += RL) {
+      float f[kCh];
+      Unit<U>::load(x, r * units + u, f);
+      welford_push(n, mean, m2, f);
+    }
+  }
+  tree_welford<kCh>(n, mean, m2, lane, CB, RL);
+  const int G = gridDim.x;
+  float* ws_mean = ws;
+  float* ws_m2 = ws + (size_t)G * C;
+  if (lane == 0 && u < units) {
+#pragma unroll
+    for (int k = 0; k < kCh; ++k) {
+      ws_mean[(size_t)blockIdx.x * C + u * kCh + k] = mean[k];
+      ws_m2[(size_t)blockIdx.x * C + u * kCh + k] = m2[k];
+    }
+  }
+  if (!last_block(counters + blockIdx.y)) return;
+
+  // The last chunk of this channel group to finish merges the group's G partials with Chan's formula for G parts:
+  // mean = sum n_g mean_g / M, M2 = sum (M2_g + n_g (mean_g - mean)^2), two fixed-order sums.
+  const Fin fin(CB);
+  const int c = blockIdx.y * fin.nc + fin.cl;
+  const bool live = c < C;
+  const float rpcf = (float)rpc, last_n = (float)(M - (size_t)(G - 1) * rpc);
+  float a = 0.f;
+  if (live) {
+#pragma unroll 8
+    for (int g = fin.sub; g < G; g += fin.tpc) a += (g == G - 1 ? last_n : rpcf) * __ldcg(ws_mean + (size_t)g * C + c);
+  }
+  const float fmean = fin.all_sum(a) / (float)M;
+  a = 0.f;
+  if (live) {
+#pragma unroll 8
+    for (int g = fin.sub; g < G; g += fin.tpc) {
+      const float d = __ldcg(ws_mean + (size_t)g * C + c) - fmean;
+      a += __ldcg(ws_m2 + (size_t)g * C + c) + (g == G - 1 ? last_n : rpcf) * d * d;
+    }
+  }
+  const float fm2 = fin.all_sum(a);
+  if (fin.sub == 0 && live) {
+    const float invstd = 1.f / sqrtf(fm2 / (float)M + eps);
+    save_mean[c] = fmean;
+    save_invstd[c] = invstd;
+    if (run_mean != nullptr) {
+      run_mean[c] = momentum * fmean + (1.f - momentum) * run_mean[c];
+      run_var[c] = momentum * (fm2 / (float)(M - 1)) + (1.f - momentum) * run_var[c];
+    }
+  }
+}
+
+template <class U, bool kRelu, bool kRes>
+__device__ __forceinline__ void fwd_row(size_t i, const float* mu, const float* sc, const float* sh, void* y,
+                                        uint8_t* mask, const float* f, const float* q) {
+  float o[kCh];
+  uint32_t bits = 0;
+#pragma unroll
+  for (int k = 0; k < kCh; ++k) {
+    float v = fmaf(f[k] - mu[k], sc[k], sh[k]);
+    if constexpr (kRes) v += q[k];
+    if constexpr (kRelu) {
+      bits |= (v > 0.f ? 1u : 0u) << k;
+      v = v <= 0.f ? 0.f : v;   // NaN propagates, as in torch.relu
+    }
+    o[k] = v;
+  }
+  Unit<U>::store(y, i, o);
+  if constexpr (kRelu) mask[i] = (uint8_t)bits;
+}
+
+template <class U, bool kRelu, bool kRes>
+__global__ void __launch_bounds__(kT, kBlocksPerSM) bn_act_fwd_apply_kernel(const void* __restrict__ x, const void* __restrict__ res,
+                                                             size_t M, int C, int shift, const float* mean,
+                                                             const float* invstd, const float* weight,
+                                                             const float* bias, void* y, uint8_t* mask) {
+  const int units = C / kCh, CB = 1 << shift, RL = kT >> shift;
+  const int col = threadIdx.x & (CB - 1), lane = threadIdx.x >> shift;
+  const int u = blockIdx.y * CB + col;
+  if (u >= units) return;
+  float mu[kCh], sc[kCh], sh[kCh];
+#pragma unroll
+  for (int k = 0; k < kCh; ++k) {
+    const int c = u * kCh + k;
+    mu[k] = mean[c];
+    sc[k] = weight[c] * invstd[c];
+    sh[k] = bias[c];
+  }
+  const size_t step = (size_t)gridDim.x * RL;
+  for (size_t r = (size_t)blockIdx.x * RL + lane; r < M; r += 2 * step) {
+    const size_t i0 = r * units + u, i1 = (r + step) * units + u;
+    const bool two = r + step < M;
+    float f0[kCh], f1[kCh], q0[kCh], q1[kCh];
+    Unit<U>::load(x, i0, f0);
+    if constexpr (kRes) Unit<U>::load(res, i0, q0);
+    if (two) {
+      Unit<U>::load(x, i1, f1);
+      if constexpr (kRes) Unit<U>::load(res, i1, q1);
+    }
+    fwd_row<U, kRelu, kRes>(i0, mu, sc, sh, y, mask, f0, q0);
+    if (two) fwd_row<U, kRelu, kRes>(i1, mu, sc, sh, y, mask, f1, q1);
+  }
+}
+
+template <bool kRelu>
+__device__ __forceinline__ void mask_grad(float* d, uint32_t bits) {
+  if constexpr (kRelu) {
+#pragma unroll
+    for (int k = 0; k < kCh; ++k) d[k] = (bits >> k) & 1u ? d[k] : 0.f;
+  }
+}
+
+template <class U, bool kRelu>
+__global__ void __launch_bounds__(kT, kBlocksPerSM) bn_act_bwd_reduce_kernel(const void* __restrict__ dy, const void* __restrict__ x,
+                                                              const uint8_t* __restrict__ mask, size_t M, int C,
+                                                              int shift, size_t rpc, const float* mean,
+                                                              const float* invstd, float* dweight, float* dbias,
+                                                              float* ws, uint32_t* counters) {
+  const int units = C / kCh, CB = 1 << shift, RL = kT >> shift;
+  const int col = threadIdx.x & (CB - 1), lane = threadIdx.x >> shift;
+  const int u = blockIdx.y * CB + col;
+  const size_t r0 = (size_t)blockIdx.x * rpc, r1 = min(M, r0 + rpc);
+  float sg[kCh], sgx[kCh], mu[kCh];
+#pragma unroll
+  for (int k = 0; k < kCh; ++k) sg[k] = sgx[k] = 0.f;
+  if (u < units) {
+#pragma unroll
+    for (int k = 0; k < kCh; ++k) mu[k] = mean[u * kCh + k];
+    size_t r = r0 + lane;
+    for (; r + 3 * RL < r1; r += 4 * RL) {
+      float d[4][kCh], f[4][kCh];
+      uint32_t bits[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const size_t i = (r + j * RL) * units + u;
+        Unit<U>::load(dy, i, d[j]);
+        Unit<U>::load(x, i, f[j]);
+        if constexpr (kRelu) bits[j] = __ldcs(mask + i);
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        mask_grad<kRelu>(d[j], bits[j]);
+#pragma unroll
+        for (int k = 0; k < kCh; ++k) {
+          sg[k] += d[j][k];
+          sgx[k] = fmaf(d[j][k], f[j][k] - mu[k], sgx[k]);
+        }
+      }
+    }
+    for (; r < r1; r += RL) {
+      const size_t i = r * units + u;
+      float d[kCh], f[kCh];
+      Unit<U>::load(dy, i, d);
+      Unit<U>::load(x, i, f);
+      if constexpr (kRelu) mask_grad<kRelu>(d, __ldcs(mask + i));
+#pragma unroll
+      for (int k = 0; k < kCh; ++k) {
+        sg[k] += d[k];
+        sgx[k] = fmaf(d[k], f[k] - mu[k], sgx[k]);
+      }
+    }
+  }
+  tree_sum2<kCh>(sg, sgx, lane, CB, RL);
+  const int G = gridDim.x;
+  float* ws_g = ws;
+  float* ws_gx = ws + (size_t)G * C;
+  if (lane == 0 && u < units) {
+#pragma unroll
+    for (int k = 0; k < kCh; ++k) {
+      ws_g[(size_t)blockIdx.x * C + u * kCh + k] = sg[k];
+      ws_gx[(size_t)blockIdx.x * C + u * kCh + k] = sgx[k];
+    }
+  }
+  if (!last_block(counters + blockIdx.y)) return;
+
+  const Fin fin(CB);
+  const int c = blockIdx.y * fin.nc + fin.cl;
+  float a = 0.f, b = 0.f;
+  if (c < C) {
+#pragma unroll 8
+    for (int g = fin.sub; g < G; g += fin.tpc) {
+      a += __ldcg(ws_g + (size_t)g * C + c);
+      b += __ldcg(ws_gx + (size_t)g * C + c);
+    }
+  }
+  tree_sum2<1>(&a, &b, fin.sub, fin.nc, fin.tpc);
+  if (fin.sub == 0 && c < C) {
+    dbias[c] = a;
+    dweight[c] = b * invstd[c];
+  }
+}
+
+template <class U, bool kRelu, bool kRes>
+__device__ __forceinline__ void bwd_row(size_t i, const float* mu, const float* A, const float* D, const float* E,
+                                        void* dx, void* dres, float* d, const float* f, uint32_t bits) {
+  mask_grad<kRelu>(d, bits);
+  float o[kCh];
+#pragma unroll
+  for (int k = 0; k < kCh; ++k) o[k] = fmaf(A[k], d[k], fmaf(D[k], f[k] - mu[k], E[k]));
+  Unit<U>::store(dx, i, o);
+  if constexpr (kRes) Unit<U>::store(dres, i, d);
+}
+
+template <class U, bool kRelu, bool kRes>
+__global__ void __launch_bounds__(kT, kBwdApplyBlocksPerSM) bn_act_bwd_apply_kernel(const void* __restrict__ dy, const void* __restrict__ x,
+                                                             const uint8_t* __restrict__ mask, size_t M, int C,
+                                                             int shift, const float* mean, const float* invstd,
+                                                             const float* weight, const float* dweight,
+                                                             const float* dbias, void* dx, void* dres) {
+  const int units = C / kCh, CB = 1 << shift, RL = kT >> shift;
+  const int col = threadIdx.x & (CB - 1), lane = threadIdx.x >> shift;
+  const int u = blockIdx.y * CB + col;
+  if (u >= units) return;
+  // dx = A * g + D * (x - mean) + E with A = w * invstd, D = -A * invstd * dweight / M, E = -A * dbias / M
+  float mu[kCh], A[kCh], D[kCh], E[kCh];
+  const float invM = 1.f / (float)M;
+#pragma unroll
+  for (int k = 0; k < kCh; ++k) {
+    const int c = u * kCh + k;
+    mu[k] = mean[c];
+    A[k] = weight[c] * invstd[c];
+    D[k] = -A[k] * invstd[c] * (dweight[c] * invM);
+    E[k] = -A[k] * (dbias[c] * invM);
+  }
+  const size_t step = (size_t)gridDim.x * RL;
+  for (size_t r = (size_t)blockIdx.x * RL + lane; r < M; r += 2 * step) {
+    const size_t i0 = r * units + u, i1 = (r + step) * units + u;
+    const bool two = r + step < M;
+    float d0[kCh], d1[kCh], f0[kCh], f1[kCh];
+    uint32_t b0 = 0, b1 = 0;
+    Unit<U>::load(dy, i0, d0);
+    Unit<U>::load(x, i0, f0);
+    if constexpr (kRelu) b0 = __ldcs(mask + i0);
+    if (two) {
+      Unit<U>::load(dy, i1, d1);
+      Unit<U>::load(x, i1, f1);
+      if constexpr (kRelu) b1 = __ldcs(mask + i1);
+    }
+    bwd_row<U, kRelu, kRes>(i0, mu, A, D, E, dx, dres, d0, f0, b0);
+    if (two) bwd_row<U, kRelu, kRes>(i1, mu, A, D, E, dx, dres, d1, f1, b1);
+  }
+}
+
+#define BN_DISPATCH_U(dtype, STMT)              \
+  switch (dtype) {                              \
+    case WIRE_F32: { using U = TagF32; STMT; } break;   \
+    case WIRE_BF16: { using U = TagBF16; STMT; } break; \
+    case WIRE_F16: { using U = TagF16; STMT; } break;   \
+    default: return cudaErrorInvalidValue;      \
+  }
+#define BN_DISPATCH_B(flag, NAME, STMT) \
+  if (flag) {                           \
+    constexpr bool NAME = true;         \
+    STMT;                               \
+  } else {                              \
+    constexpr bool NAME = false;        \
+    STMT;                               \
+  }
+
+bool aligned16(const void* p) { return ((uintptr_t)p & 15u) == 0; }
+
+bool bad_shape(size_t M, int C) { return M < 1 || C < kCh || C % kCh != 0; }
+
+int apply_grid(size_t M, const Geo& g, int per_sm) {
+  const size_t want = (size_t)(wave_blocks(per_sm) / g.ncb > 0 ? wave_blocks(per_sm) / g.ncb : 1);
+  const size_t most = (M + 2 * (size_t)g.rl - 1) / (2 * (size_t)g.rl);
+  return (int)(most < want ? (most < 1 ? 1 : most) : want);
+}
+
+}  // namespace
+
+size_t bn_act_workspace_floats(size_t M, int C) {
+  size_t rpc;
+  int G;
+  chunks(M, geo(C, red_cb(C)), &rpc, &G);
+  return 2 * (size_t)G * (size_t)C;
+}
+
+int bn_act_counters(int C) { return geo(C, red_cb(C)).ncb; }
+
+cudaError_t launch_bn_act_fwd_stats(const void* x, int dtype, size_t M, int C, float eps, float momentum,
+                                    float* running_mean, float* running_var, float* save_mean, float* save_invstd,
+                                    float* ws, uint32_t* counters, cudaStream_t s) {
+  if (bad_shape(M, C) || M < 2 || !aligned16(x) || (running_mean == nullptr) != (running_var == nullptr))
+    return cudaErrorInvalidValue;
+  const Geo g = geo(C, red_cb(C));
+  size_t rpc;
+  int G;
+  chunks(M, g, &rpc, &G);
+  const dim3 grid(G, g.ncb);
+  BN_DISPATCH_U(dtype, (bn_act_fwd_stats_kernel<U><<<grid, kT, 0, s>>>(x, M, C, g.shift, rpc, eps, momentum,
+                                                                        running_mean, running_var, save_mean,
+                                                                        save_invstd, ws, counters)));
+  return cudaGetLastError();
+}
+
+cudaError_t launch_bn_act_fwd_apply(const void* x, const void* residual, int dtype, size_t M, int C, const float* mean,
+                                    const float* invstd, const float* weight, const float* bias, int relu, void* y,
+                                    uint8_t* mask, cudaStream_t s) {
+  if (bad_shape(M, C) || !aligned16(x) || !aligned16(residual) || !aligned16(y) || (relu && mask == nullptr))
+    return cudaErrorInvalidValue;
+  const Geo g = geo(C, kMaxCB);
+  const dim3 grid(apply_grid(M, g, kBlocksPerSM), g.ncb);
+  BN_DISPATCH_U(dtype, BN_DISPATCH_B(relu, kRelu, BN_DISPATCH_B(residual != nullptr, kRes, (
+      bn_act_fwd_apply_kernel<U, kRelu, kRes><<<grid, kT, 0, s>>>(x, residual, M, C, g.shift, mean, invstd, weight,
+                                                                  bias, y, mask)))));
+  return cudaGetLastError();
+}
+
+cudaError_t launch_bn_act_bwd_reduce(const void* dy, const void* x, const uint8_t* mask, int dtype, size_t M, int C,
+                                     const float* mean, const float* invstd, float* dweight, float* dbias, float* ws,
+                                     uint32_t* counters, cudaStream_t s) {
+  if (bad_shape(M, C) || !aligned16(dy) || !aligned16(x)) return cudaErrorInvalidValue;
+  const Geo g = geo(C, red_cb(C));
+  size_t rpc;
+  int G;
+  chunks(M, g, &rpc, &G);
+  const dim3 grid(G, g.ncb);
+  BN_DISPATCH_U(dtype, BN_DISPATCH_B(mask != nullptr, kRelu, (
+      bn_act_bwd_reduce_kernel<U, kRelu><<<grid, kT, 0, s>>>(dy, x, mask, M, C, g.shift, rpc, mean, invstd, dweight,
+                                                             dbias, ws, counters))));
+  return cudaGetLastError();
+}
+
+cudaError_t launch_bn_act_bwd_apply(const void* dy, const void* x, const uint8_t* mask, int dtype, size_t M, int C,
+                                    const float* mean, const float* invstd, const float* weight, const float* dweight,
+                                    const float* dbias, void* dx, void* dresidual, cudaStream_t s) {
+  if (bad_shape(M, C) || !aligned16(dy) || !aligned16(x) || !aligned16(dx) || !aligned16(dresidual))
+    return cudaErrorInvalidValue;
+  const Geo g = geo(C, kMaxCB);
+  const dim3 grid(apply_grid(M, g, kBwdApplyBlocksPerSM), g.ncb);
+  BN_DISPATCH_U(dtype, BN_DISPATCH_B(mask != nullptr, kRelu, BN_DISPATCH_B(dresidual != nullptr, kRes, (
+      bn_act_bwd_apply_kernel<U, kRelu, kRes><<<grid, kT, 0, s>>>(dy, x, mask, M, C, g.shift, mean, invstd, weight,
+                                                                  dweight, dbias, dx, dresidual)))));
+  return cudaGetLastError();
+}
+
+}  // namespace bps

@@ -147,6 +147,23 @@ __device__ __forceinline__ void barrier_peers(const PeerView& pv, int channel) {
   if (threadIdx.x == 0) pv.epoch[slot_base] += 1;
 }
 
+// "Last block out" pattern: returns true (for the whole block) in the block that arrives last among the gridDim.x
+// blocks counting on `counter`, after every earlier block's global writes are visible.  The counter is reset to 0
+// by that block, so it is ready for the next launch on the same stream.
+__device__ __forceinline__ bool last_block(uint32_t* counter) {
+  __shared__ uint32_t s_last;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    const uint32_t prev = atomicAdd(counter, 1u);
+    s_last = prev == gridDim.x - 1 ? 1u : 0u;
+    if (s_last) *counter = 0;
+    __threadfence();
+  }
+  __syncthreads();
+  return s_last != 0;
+}
+
 // ---- numeric packing ----------------------------------------------------------
 __device__ __forceinline__ float2 bf16x2_to_f2(uint32_t u) {
   return make_float2(__uint_as_float(u << 16), __uint_as_float(u & 0xffff0000u));

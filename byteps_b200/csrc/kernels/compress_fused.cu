@@ -50,21 +50,6 @@ __device__ __forceinline__ float block_sum(float v) {
   return r;
 }
 
-// "last block out" pattern: returns true (for the whole block) in the block that arrives last.
-__device__ __forceinline__ bool last_block(uint32_t* counter) {
-  __shared__ uint32_t s_last;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    const uint32_t prev = atomicAdd(counter, 1u);
-    s_last = prev == gridDim.x - 1 ? 1u : 0u;
-    if (s_last) *counter = 0;
-    __threadfence();
-  }
-  __syncthreads();
-  return s_last != 0;
-}
-
 // fixed-order sum of `nparts` block partials by one block; result in thread 0
 __device__ __forceinline__ float sum_partials(const float* parts, int nparts) {
   float a = 0.f;

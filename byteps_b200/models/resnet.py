@@ -3,6 +3,8 @@ reference's headline synthetic benchmark."""
 import torch
 import torch.nn as nn
 
+from ..ops.bn_act import BatchNormAct2d
+
 
 def _conv3x3(i, o, stride=1):
     return nn.Conv2d(i, o, 3, stride, 1, bias=False)
@@ -18,17 +20,15 @@ class BasicBlock(nn.Module):
     def __init__(self, inplanes, planes, stride=1, downsample=None):
         super().__init__()
         self.conv1 = _conv3x3(inplanes, planes, stride)
-        self.bn1 = nn.BatchNorm2d(planes)
+        self.bn1 = BatchNormAct2d(planes, act="relu")
         self.conv2 = _conv3x3(planes, planes)
-        self.bn2 = nn.BatchNorm2d(planes)
-        self.relu = nn.ReLU(inplace=True)
+        self.bn2 = BatchNormAct2d(planes, act="relu")
         self.downsample = downsample
 
     def forward(self, x):
         idt = x if self.downsample is None else self.downsample(x)
-        out = self.relu(self.bn1(self.conv1(x)))
-        out = self.bn2(self.conv2(out))
-        return self.relu(out + idt)
+        out = self.bn1(self.conv1(x))
+        return self.bn2(self.conv2(out), idt)
 
 
 class Bottleneck(nn.Module):
@@ -37,20 +37,18 @@ class Bottleneck(nn.Module):
     def __init__(self, inplanes, planes, stride=1, downsample=None):
         super().__init__()
         self.conv1 = _conv1x1(inplanes, planes)
-        self.bn1 = nn.BatchNorm2d(planes)
+        self.bn1 = BatchNormAct2d(planes, act="relu")
         self.conv2 = _conv3x3(planes, planes, stride)
-        self.bn2 = nn.BatchNorm2d(planes)
+        self.bn2 = BatchNormAct2d(planes, act="relu")
         self.conv3 = _conv1x1(planes, planes * 4)
-        self.bn3 = nn.BatchNorm2d(planes * 4)
-        self.relu = nn.ReLU(inplace=True)
+        self.bn3 = BatchNormAct2d(planes * 4, act="relu")
         self.downsample = downsample
 
     def forward(self, x):
         idt = x if self.downsample is None else self.downsample(x)
-        out = self.relu(self.bn1(self.conv1(x)))
-        out = self.relu(self.bn2(self.conv2(out)))
-        out = self.bn3(self.conv3(out))
-        return self.relu(out + idt)
+        out = self.bn1(self.conv1(x))
+        out = self.bn2(self.conv2(out))
+        return self.bn3(self.conv3(out), idt)
 
 
 class ResNet(nn.Module):
@@ -58,8 +56,7 @@ class ResNet(nn.Module):
         super().__init__()
         self.inplanes = 64
         self.conv1 = nn.Conv2d(3, 64, 7, 2, 3, bias=False)
-        self.bn1 = nn.BatchNorm2d(64)
-        self.relu = nn.ReLU(inplace=True)
+        self.bn1 = BatchNormAct2d(64, act="relu")
         self.maxpool = nn.MaxPool2d(3, 2, 1)
         self.layer1 = self._make_layer(block, 64, layers[0])
         self.layer2 = self._make_layer(block, 128, layers[1], 2)
@@ -84,14 +81,14 @@ class ResNet(nn.Module):
         down = None
         if stride != 1 or self.inplanes != planes * block.expansion:
             down = nn.Sequential(_conv1x1(self.inplanes, planes * block.expansion, stride),
-                                 nn.BatchNorm2d(planes * block.expansion))
+                                 BatchNormAct2d(planes * block.expansion))
         layers = [block(self.inplanes, planes, stride, down)]
         self.inplanes = planes * block.expansion
         layers += [block(self.inplanes, planes) for _ in range(1, blocks)]
         return nn.Sequential(*layers)
 
     def forward(self, x):
-        x = self.maxpool(self.relu(self.bn1(self.conv1(x))))
+        x = self.maxpool(self.bn1(self.conv1(x)))
         x = self.layer4(self.layer3(self.layer2(self.layer1(x))))
         return self.fc(torch.flatten(self.avgpool(x), 1))
 
