@@ -54,6 +54,41 @@ def _dense(p: torch.Tensor) -> bool:
     return span == p.numel()
 
 
+def shard_bounds(numel: int, world: int, rank: int):
+    """Element range [begin, end) of the shard `rank` owns in a bucket of `numel` (padded) elements: the bucket
+    is cut into `world` equal runs of 8-element units; trailing ranks of a small bucket own an empty shard."""
+    units = numel // 8
+    per = (units + world - 1) // world
+    s0 = min(per * rank, units)
+    s1 = min(s0 + per, units)
+    return s0 * 8, s1 * 8
+
+
+def copy_bucket_state(shard: torch.Tensor, span, starts: List[int], tensors: List[torch.Tensor], to_shard: bool):
+    """Copy between one shard of a bucket's flat state and per-parameter tensors - the one place that knows how
+    the optimizer state of a bucket is laid out.
+
+    `shard` holds elements [span[0], span[1]) of the flat bucket layout: parameter i occupies
+    [starts[i], starts[i] + numel) in storage order (as `_strided_view` maps it, so a channels_last weight is
+    stored NHWC), padded to a multiple of 8 elements.  `tensors[i]` has parameter i's shape AND strides, so its
+    own storage order is the bucket's.  to_shard=True scatters the tensors into the shard and leaves every
+    element no parameter covers (padding, the tail of an over-allocated shard) zero; to_shard=False gathers the
+    shard's part of each parameter into its tensor and leaves the rest of the tensor as it was."""
+    s0, s1 = span
+    if to_shard:
+        shard.zero_()
+    for t, st in zip(tensors, starts):
+        n = t.numel()
+        lo, hi = max(st, s0), min(st + n, s1)
+        if lo >= hi:
+            continue
+        flat = torch.as_strided(t, (n,), (1,), t.storage_offset())
+        if to_shard:
+            shard[lo - s0:hi - s0].copy_(flat[lo - st:hi - st])
+        else:
+            flat[lo - st:hi - st].copy_(shard[lo - s0:hi - s0])
+
+
 @dataclass
 class Bucket:
     index: int
@@ -235,11 +270,7 @@ class BucketedGradSync:
 
     def shard_range(self, b: Bucket):
         """Element range [begin, end) of the shard this rank owns in bucket b."""
-        units = b.numel // 8
-        per = (units + self.world - 1) // self.world
-        s0 = min(per * self.rank, units)
-        s1 = min(s0 + per, units)
-        return s0 * 8, s1 * 8
+        return shard_bounds(b.numel, self.world, self.rank)
 
     # ------------------------------------------------------------------ fused optimizer state
     def _init_fused_state(self):
@@ -781,6 +812,73 @@ class BucketedGradSync:
                 if lo < hi:
                     out[p] = (lo - st, b.master[lo - s0:hi - s0])
         return out
+
+    _STATE_KEYS = ("master", "state0", "state1")
+
+    def export_state(self) -> Dict[torch.nn.Parameter, Dict[str, torch.Tensor]]:
+        """The full fp32 optimizer state, {param: {"master", "state0"[, "state1"]: CPU tensor}}, each tensor with
+        its parameter's shape and strides.  Collective when world > 1: every rank must call it, and every rank
+        gets the whole state.  Per bucket and buffer, this rank's shard goes into a zero host buffer of the
+        bucket's length, and the buffers' bit patterns are summed over ranks as int32 through the engine's host
+        collective, one bucket at a time.  Every element is non-zero on one rank at most, so the sum reproduces each
+        rank's bits exactly (negative zeros and NaN payloads included); no float arithmetic and no wire cast
+        (BYTEPS_WIRE_DTYPE applies to float32 exchanges on the device) touches the state."""
+        if not self.fused:
+            raise RuntimeError("export_state needs the fused optimizer")
+        out: Dict[torch.nn.Parameter, Dict[str, torch.Tensor]] = {p: {} for b in self.buckets for p in b.params}
+        for b in self.buckets:
+            s0, s1 = self.shard_range(b)
+            for key in self._STATE_KEYS:
+                buf = getattr(b, key)
+                if buf is None:
+                    continue
+                host = torch.zeros(b.numel, dtype=torch.float32)
+                host[s0:s1].copy_(buf[:s1 - s0])
+                if self.world > 1:
+                    bits = host.view(torch.int32)
+                    h = self.engine.push_pull_async(bits, bits, False, "FusedState.%d.%d.%s" % (b.index, b.numel, key))
+                    self.engine.synchronize(h)
+                tensors = [torch.empty_strided(p.size(), p.stride(), dtype=torch.float32) for p in b.params]
+                copy_bucket_state(host, (0, b.numel), b.starts, tensors, to_shard=False)
+                for p, t in zip(b.params, tensors):
+                    out[p][key] = t
+        return out
+
+    def import_state(self, state: Dict[torch.nn.Parameter, Dict[str, torch.Tensor]], group_steps: List[int]):
+        """Install full per-parameter state (as `export_state` returns it; any shape-matching dtype and layout)
+        and the per-group step counts.  Each rank copies its own slice IN PLACE into the existing shard buffers,
+        whose addresses a captured CUDA graph or ring table may hold.  A missing entry takes the initial value:
+        the master from the current parameter, zero moments / momentum."""
+        if not self.fused:
+            raise RuntimeError("import_state needs the fused optimizer")
+        if len(group_steps) != len(self._group_step):
+            raise ValueError("expected %d group step counts, got %d" % (len(self._group_step), len(group_steps)))
+        for p, ent in state.items():
+            for key, v in ent.items():
+                if v is not None and tuple(v.shape) != tuple(p.shape):
+                    raise ValueError("state %r has shape %s, its parameter %s" % (key, tuple(v.shape), tuple(p.shape)))
+        for b in self.buckets:
+            s0, s1 = self.shard_range(b)
+            for key in self._STATE_KEYS:
+                buf = getattr(b, key)
+                if buf is None:
+                    continue
+                tensors = []
+                for p in b.params:
+                    v = state.get(p, {}).get(key)
+                    t = torch.empty_strided(p.size(), p.stride(), dtype=torch.float32)
+                    if v is not None:
+                        t.copy_(v)
+                    elif key == "master":
+                        t.copy_(p.detach())
+                    else:
+                        t.zero_()
+                    tensors.append(t)
+                stage = torch.empty(buf.numel(), dtype=torch.float32)
+                copy_bucket_state(stage, (s0, s1), b.starts, tensors, to_shard=True)
+                buf.copy_(stage)
+        self._group_step = [int(t) for t in group_steps]
+        self.refresh_hparams()
 
     def close(self):
         self.remove_hooks()

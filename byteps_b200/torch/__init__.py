@@ -235,6 +235,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         so lr/momentum/Adam bias corrections of that step reach the kernels
         (eager ``step()`` does the equivalent by itself)."""
         if self._sync is not None:
+            self._drop_loaded_state()
             self._sync.pre_replay()
 
     def step(self, closure=None):
@@ -257,6 +258,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             self.synchronize()
             return loss
         if self._fused:
+            self._drop_loaded_state()
             loss = closure() if closure is not None else None
             # the update already happened inside the exchange kernels
             if self._should_sync:
@@ -272,6 +274,101 @@ class _DistributedOptimizer(torch.optim.Optimizer):
     @property
     def grad_sync(self):
         return self._sync
+
+    def _drop_loaded_state(self):
+        """Fused mode: forget the full copies of a load that no broadcast_optimizer_state consumed.  Training has
+        moved on from them (a later broadcast must offer the live state, not roll back to the checkpoint)."""
+        if self._fused and self.state:
+            self.state.clear()
+
+    # ---- checkpoints of the fused optimizer ----------------------------------------
+    # With fused_update the state lives in the exchange's fp32 shards, not in self.state.  state_dict() gathers it
+    # into the layout torch.optim uses (SGD: momentum_buffer; Adam/AdamW: step, exp_avg, exp_avg_sq), plus
+    # master_param for 16-bit parameters; load_state_dict() takes that layout, from this class or from torch.optim.
+    _FUSED_KEYS = {"sgd": ("momentum_buffer",), "adam": ("exp_avg", "exp_avg_sq"), "adamw": ("exp_avg", "exp_avg_sq")}
+
+    def state_dict(self):
+        """The optimizer state in ``torch.optim``'s format.
+
+        With ``fused_update=True`` and more than one process this call is collective, like FSDP's optimizer
+        state dict: every rank must call it (and every rank gets the full state); save it on one rank only.
+        The state is full, not sharded, so it loads at any world size and into a plain ``torch.optim``
+        optimizer.  Tensors are fp32 CPU tensors with their parameter's shape and strides.  16-bit parameters
+        get one extra entry, ``master_param``, the fp32 master weights.
+        """
+        sd = super(self.__class__, self).state_dict()
+        if not self._fused:
+            return sd
+        full = self._sync.export_state()
+        state = {}
+        idx = 0
+        for gi, g in enumerate(self.param_groups):
+            t = self._sync._group_step[gi]
+            for p in g["params"]:
+                ent = full.get(p)
+                if ent is not None:
+                    e = {}
+                    if t > 0 and self._fused == "sgd":
+                        if g.get("momentum", 0) != 0:
+                            e["momentum_buffer"] = ent["state0"]
+                    elif t > 0:
+                        e["step"] = torch.tensor(float(t), dtype=torch.float32)
+                        e["exp_avg"], e["exp_avg_sq"] = ent["state0"], ent["state1"]
+                    # torch's Adam creates its state only for a parameter without any: an entry holding only the
+                    # masters (nothing has been stepped yet, so they equal the weights) would stop it
+                    if p.dtype != torch.float32 and (t > 0 or self._fused == "sgd"):
+                        e["master_param"] = ent["master"]
+                    if e:
+                        state[idx] = e
+                idx += 1
+        sd["state"] = state
+        return sd
+
+    def load_state_dict(self, state_dict):
+        """Load a state dict of ``state_dict()`` or of the matching ``torch.optim`` optimizer.
+
+        With ``fused_update=True`` the state is copied in place into this rank's shards (CUDA graphs captured
+        earlier stay valid) and the full tensors are also kept in ``self.state`` until
+        ``broadcast_optimizer_state`` hands them to the other ranks, so loading on rank 0 only works.  The next
+        ``step()`` (or ``refresh_hparams()`` before a graph replay) drops them if no broadcast came first.  A
+        ``momentum_buffer`` means SGD has taken a step; Adam's ``step`` must be equal within a param group.
+        Missing entries start fresh: master weights from the current parameters (load the model first),
+        zero moments.
+        """
+        if not self._fused:
+            return super(self.__class__, self).load_state_dict(state_dict)
+        live = [p for g in self.param_groups for p in g["params"]]
+        saved = [i for g in state_dict["param_groups"] for i in g["params"]]
+        by_id = dict(zip(saved, live))
+        full = {}
+        for i, ent in state_dict["state"].items():
+            p = by_id.get(i)
+            if p is None:
+                continue
+            full[p] = {k: (_full_like(p, v) if torch.is_tensor(v) and v.dim() > 0 else v) for k, v in ent.items()}
+        steps = []
+        for g in self.param_groups:
+            ents = [full[p] for p in g["params"] if p in full]
+            if self._fused == "sgd":
+                steps.append(1 if any("momentum_buffer" in e for e in ents) else 0)
+                continue
+            vals = sorted({float(e["step"]) for e in ents if "step" in e})
+            if len(vals) > 1:
+                raise ValueError("loaded state dict has different Adam step counts in one parameter group: %s"
+                                 % vals)
+            steps.append(int(vals[0]) if vals else 0)
+        # torch rebuilds param_groups as new dicts: put the loaded options into the live ones instead, which the
+        # wrapped optimizer and the exchange's hyper-parameter feed hold
+        groups = self.param_groups
+        super(self.__class__, self).load_state_dict({"state": {}, "param_groups": state_dict["param_groups"]})
+        for old, new in zip(groups, self.param_groups):
+            old.update(new)
+        self.param_groups = groups
+        self.state.update(full)
+        keys = self._FUSED_KEYS[self._fused]
+        self._sync.import_state({p: dict({"master": e.get("master_param")},
+                                         **{"state%d" % i: e.get(k) for i, k in enumerate(keys)})
+                                 for p, e in full.items()}, steps)
 
 
 def DistributedOptimizer(optimizer, named_parameters=None, compression=Compression.none,
@@ -332,12 +429,46 @@ def _dense_tensor(t):
     return span == t.numel()
 
 
-def _materialised_state(optimizer):
+def _full_like(p, value=None):
+    """An fp32 CPU tensor with p's shape and strides holding `value` (zeros if None).  Every rank lays the
+    state tensors of a broadcast out like this, so their flat storage views line up."""
+    t = torch.empty_strided(p.size(), p.stride(), dtype=torch.float32)
+    if value is None:
+        return t.zero_()
+    if tuple(value.shape) != tuple(p.shape):
+        raise ValueError("loaded state of shape %s for a parameter of shape %s"
+                         % (tuple(value.shape), tuple(p.shape)))
+    return t.copy_(value)
+
+
+def _fused_broadcast_source(optimizer, root_rank):
+    """Fused mode: the state dict every rank feeds into the in-place broadcast.  A root that loaded a state dict
+    offers the full tensors load_state_dict() kept in ``optimizer.state``, and the other ranks zero tensors of the
+    same keys, shapes and strides.  A root that loaded nothing offers its live state, which every rank exports
+    together (after the layout's broadcast has re-derived the masters from the parameters)."""
+    base = super(optimizer.__class__, optimizer).state_dict()     # param_groups, and what self.state holds
+    layout = None
+    if rank() == root_rank and base["state"]:
+        layout = {i: {k: torch.is_tensor(v) and v.dim() > 0 for k, v in ent.items()}
+                  for i, ent in base["state"].items()}
+    layout = broadcast_object(layout, root_rank, name="optimizer_state.layout")
+    if layout is None:
+        return optimizer.state_dict()
+    if rank() != root_rank:
+        live = [p for g in optimizer.param_groups for p in g["params"]]
+        base["state"] = {i: {k: _full_like(live[i]) if is_tensor else torch.tensor(0.0)
+                             for k, is_tensor in ent.items()} for i, ent in layout.items()}
+    return base
+
+
+def _materialised_state(optimizer, root_rank=0):
     """state_dict of an optimizer whose per-parameter state exists.  A fresh optimizer has none until its first
     step: take one step of the INNER optimizer on zero gradients and undo whatever it did to the weights
     (weight decay moves them even with a zero gradient)."""
+    if getattr(optimizer, "_fused", None):
+        return _fused_broadcast_source(optimizer, root_rank)
     sd = optimizer.state_dict()
-    if sd["state"] or getattr(optimizer, "_fused", None):
+    if sd["state"]:
         return sd
     weights = [p for g in optimizer.param_groups for p in g["params"]]
     for p in weights:
@@ -355,11 +486,18 @@ def broadcast_optimizer_state(optimizer, root_rank, prefix="Parameter."):
     """Make every process's optimizer state equal to ``root_rank``'s: tensor entries (momentum buffers, Adam
     moments, ...) are broadcast in place like parameters, everything else - python / 0-dim state entries such as
     ``step`` and the options of every param group (lr, betas, ...) - travels as one pickled tree.
-    (Reference: byteps/torch/__init__.py:302-424.)"""
+    (Reference: byteps/torch/__init__.py:302-424.)
+
+    With ``fused_update=True`` the root's state is what its last ``load_state_dict`` loaded (so loading on the
+    root only is enough), or else its live state.  Every rank installs its shard of it, and the full copies
+    ``load_state_dict`` kept are dropped.  ``broadcast_parameters`` re-derives the fp32 master weights from the
+    parameters, so call it first: this call then puts the loaded masters back.  Without a loaded state the
+    masters stay re-derived from the parameters, as after any ``broadcast_parameters``."""
     if isinstance(optimizer, torch.optim.LBFGS):
         raise ValueError("cannot broadcast torch.optim.LBFGS state")
-    sd = _materialised_state(optimizer)
-    if not sd["state"]:
+    fused = getattr(optimizer, "_fused", None)
+    sd = _materialised_state(optimizer, root_rank)
+    if not sd["state"] and not fused:
         return
     tensors = []                                     # (name, tensor); names are equal on all ranks by construction
     plain = {"groups": [{k: v for k, v in g.items() if k != "params"} for g in sd["param_groups"]], "state": {}}
@@ -380,6 +518,8 @@ def broadcast_optimizer_state(optimizer, root_rank, prefix="Parameter."):
     # tensors were overwritten in place; the plain entries reach the optimizer through load_state_dict (torch
     # casts a python `step` back to the tensor form the optimizer keeps)
     optimizer.load_state_dict(sd)
+    if fused:
+        optimizer.state.clear()         # every rank holds its shard now
 
 
 def broadcast_object(obj, root_rank=0, name=None):

@@ -4,7 +4,11 @@
 saves/loads with torch.save/load, everybody receives the state through
 broadcast_parameters + broadcast_optimizer_state; gradient accumulation with
 backward_passes_per_step; lr warm-up; metrics averaged by push_pull.  Synthetic
-data stands in for the dataset (no network)."""
+data stands in for the dataset (no network).
+
+With --fused-update the optimizer state lives in per-rank shards of the exchange; its
+state_dict() gathers the full state and is collective, so every rank calls it and
+rank 0 alone saves."""
 import argparse
 import os
 import sys
@@ -27,6 +31,7 @@ p.add_argument("--warmup-epochs", type=float, default=1)
 p.add_argument("--model", default="resnet50")
 p.add_argument("--image-size", type=int, default=224)
 p.add_argument("--no-cuda", action="store_true")
+p.add_argument("--fused-update", action="store_true", help="SGD step inside the exchange kernel (fp32 master shards)")
 args = p.parse_args()
 bps.init()
 cuda = torch.cuda.is_available() and not args.no_cuda
@@ -43,7 +48,8 @@ model = get_model(args.model).to(dev)
 opt = torch.optim.SGD(model.parameters(), lr=args.base_lr * args.batches_per_pushpull * bps.size(), momentum=0.9,
                       weight_decay=5e-5)
 opt = bps.DistributedOptimizer(opt, named_parameters=model.named_parameters(),
-                               backward_passes_per_step=args.batches_per_pushpull)
+                               backward_passes_per_step=args.batches_per_pushpull,
+                               fused_update=args.fused_update and cuda)
 if resume_from > 0 and bps.rank() == 0:
     ck = torch.load(args.checkpoint_format.format(epoch=resume_from), map_location=dev)
     model.load_state_dict(ck["model"])
@@ -64,8 +70,8 @@ for epoch in range(resume_from, args.epochs):
             loss.backward()
         opt.step()
     avg = bps.push_pull(loss.detach(), name="train_loss").item()
+    opt_state = opt.state_dict()            # collective with --fused-update: every rank takes part
     if bps.rank() == 0:
         print("epoch %d: avg loss %.4f%s" % (epoch + 1, avg, " (resumed from epoch %d)" % resume_from if resume_from else ""))
-        torch.save({"model": model.state_dict(), "optimizer": opt.state_dict()},
-                   args.checkpoint_format.format(epoch=epoch + 1))
+        torch.save({"model": model.state_dict(), "optimizer": opt_state}, args.checkpoint_format.format(epoch=epoch + 1))
 bps.shutdown()
