@@ -48,11 +48,40 @@ void bind_cuda_bn(py::module_& m) {
   });
   m.def("bn_act_bwd_apply", [](uintptr_t dy, uintptr_t x, uintptr_t mask, int dtype, size_t M, int C, uintptr_t mean,
                                uintptr_t invstd, uintptr_t weight, uintptr_t dweight, uintptr_t dbias, uintptr_t dx,
-                               uintptr_t dresidual, uintptr_t s) {
+                               uintptr_t dresidual, uintptr_t s, uintptr_t total) {
     chk(launch_bn_act_bwd_apply((const void*)dy, (const void*)x, (const uint8_t*)mask, dtype, M, C,
                                 (const float*)mean, (const float*)invstd, (const float*)weight,
                                 (const float*)dweight, (const float*)dbias, (void*)dx, (void*)dresidual,
-                                (cudaStream_t)s),
+                                (cudaStream_t)s, (const float*)total),
         "bn_act_bwd_apply");
+  }, py::arg("dy"), py::arg("x"), py::arg("mask"), py::arg("dtype"), py::arg("M"), py::arg("C"), py::arg("mean"),
+     py::arg("invstd"), py::arg("weight"), py::arg("dweight"), py::arg("dbias"), py::arg("dx"), py::arg("dresidual"),
+     py::arg("stream"), py::arg("total") = 0,
+     "total: device float holding the row count to divide by (bn_sync_stats writes it); 0 divides by M");
+
+  // ---- synchronised batch norm
+  m.def("bn_act_load_kernels", []() { chk(bn_act_load_kernels(), "bn_act_load_kernels"); },
+        "load every batch-norm kernel variant now (before any cross-rank launch)");
+  m.def("bn_sync_window_floats", &bn_sync_window_floats, py::arg("world"), py::arg("cmax"));
+  m.def("bn_act_fwd_stats_local", [](uintptr_t x, int dtype, size_t M, int C, uintptr_t local_mean,
+                                     uintptr_t local_m2, uintptr_t ws, uintptr_t counters, uintptr_t s) {
+    chk(launch_bn_act_fwd_stats_local((const void*)x, dtype, M, C, (float*)local_mean, (float*)local_m2, (float*)ws,
+                                      (uint32_t*)counters, (cudaStream_t)s),
+        "bn_act_fwd_stats_local");
+  });
+  m.def("bn_sync_stats", [](const PeerView& pv, int channel, size_t win_off, int cmax, int C, uintptr_t local_mean,
+                            uintptr_t local_m2, float count, float eps, float momentum, uintptr_t running_mean,
+                            uintptr_t running_var, uintptr_t save_mean, uintptr_t save_invstd, uintptr_t total,
+                            uintptr_t s) {
+    chk(launch_bn_sync_stats(pv, channel, win_off, cmax, C, (const float*)local_mean, (const float*)local_m2, count,
+                             eps, momentum, (float*)running_mean, (float*)running_var, (float*)save_mean,
+                             (float*)save_invstd, (float*)total, (cudaStream_t)s),
+        "bn_sync_stats");
+  });
+  m.def("bn_sync_grad", [](const PeerView& pv, int channel, size_t win_off, int cmax, int C, uintptr_t dbias,
+                           uintptr_t dweight, uintptr_t sum_dbias, uintptr_t sum_dweight, uintptr_t s) {
+    chk(launch_bn_sync_grad(pv, channel, win_off, cmax, C, (const float*)dbias, (const float*)dweight,
+                            (float*)sum_dbias, (float*)sum_dweight, (cudaStream_t)s),
+        "bn_sync_grad");
   });
 }

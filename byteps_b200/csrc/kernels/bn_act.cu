@@ -182,7 +182,9 @@ struct Fin {
   }
 };
 
-template <class U>
+// kLocal: local-partials mode of synchronised batch norm - save_mean / save_invstd receive this rank's mean and
+// M2 over its M rows (M >= 1), and the running statistics are left to bn_sync_kernel.
+template <class U, bool kLocal>
 __global__ void __launch_bounds__(kT, kBlocksPerSM) bn_act_fwd_stats_kernel(const void* __restrict__ x, size_t M, int C, int shift,
                                                              size_t rpc, float eps, float momentum, float* run_mean,
                                                              float* run_var, float* save_mean, float* save_invstd,
@@ -243,7 +245,12 @@ __global__ void __launch_bounds__(kT, kBlocksPerSM) bn_act_fwd_stats_kernel(cons
     }
   }
   const float fm2 = fin.all_sum(a);
-  if (fin.sub == 0 && live) {
+  if constexpr (kLocal) {
+    if (fin.sub == 0 && live) {
+      save_mean[c] = fmean;
+      save_invstd[c] = fm2;
+    }
+  } else if (fin.sub == 0 && live) {
     const float invstd = 1.f / sqrtf(fm2 / (float)M + eps);
     save_mean[c] = fmean;
     save_invstd[c] = invstd;
@@ -405,19 +412,22 @@ __device__ __forceinline__ void bwd_row(size_t i, const float* mu, const float* 
   if constexpr (kRes) Unit<U>::store(dres, i, d);
 }
 
-template <class U, bool kRelu, bool kRes>
+// kTotal: divide by *total, the row count of all ranks (synchronised batch norm), instead of M.
+template <class U, bool kRelu, bool kRes, bool kTotal>
 __global__ void __launch_bounds__(kT, kBwdApplyBlocksPerSM) bn_act_bwd_apply_kernel(const void* __restrict__ dy, const void* __restrict__ x,
                                                              const uint8_t* __restrict__ mask, size_t M, int C,
                                                              int shift, const float* mean, const float* invstd,
                                                              const float* weight, const float* dweight,
-                                                             const float* dbias, void* dx, void* dres) {
+                                                             const float* dbias, void* dx, void* dres,
+                                                             const float* total) {
   const int units = C / kCh, CB = 1 << shift, RL = kT >> shift;
   const int col = threadIdx.x & (CB - 1), lane = threadIdx.x >> shift;
   const int u = blockIdx.y * CB + col;
   if (u >= units) return;
-  // dx = A * g + D * (x - mean) + E with A = w * invstd, D = -A * invstd * dweight / M, E = -A * dbias / M
+  // dx = A * g + D * (x - mean) + E with A = w * invstd, D = -A * invstd * dweight / N, E = -A * dbias / N, where
+  // N is the row count of the statistics
   float mu[kCh], A[kCh], D[kCh], E[kCh];
-  const float invM = 1.f / (float)M;
+  const float invM = 1.f / (kTotal ? *total : (float)M);
 #pragma unroll
   for (int k = 0; k < kCh; ++k) {
     const int c = u * kCh + k;
@@ -442,6 +452,91 @@ __global__ void __launch_bounds__(kT, kBwdApplyBlocksPerSM) bn_act_bwd_apply_ker
     }
     bwd_row<U, kRelu, kRes>(i0, mu, A, D, E, dx, dres, d0, f0, b0);
     if (two) bwd_row<U, kRelu, kRes>(i1, mu, A, D, E, dx, dres, d1, f1, b1);
+  }
+}
+
+// ---- synchronised batch norm: the cross-rank step between the local reduction and the apply pass -------------
+//
+// Window of one rank (float offsets from its base): slot (parity p, source rank r) at (p * W + r) * slot, with
+// slot = kSyncPad + 2 * cmax floats: [counts: one 16-byte vector per block][a: cmax][b: cmax].  Block k owns the
+// channel steps k, k + gridDim.x, ... of kSyncStep channels.  gridDim.x is min(steps, kMaxSyncBlocks), so step j
+// is always owned by block j % kMaxSyncBlocks whatever C is, and a window area is only ever written by blocks
+// with one blockIdx.x, under that block's barrier generation.
+//
+// Slot reuse.  A block works in the slots of parity g & 1, g being its barrier generation in device memory
+// (epoch[channel][block]); every rank runs the same sequence of sync launches, so the counterparts of a block on
+// all ranks are at the same generation when they meet.  The block of participation j on rank A writes A's slot in
+// every peer's window before barrier j, and reads its own window after it.  A peer block can be at most one
+// participation ahead: to pass barrier j + 1 it needs this block at j + 1, which this rank's stream starts only
+// after participation j has finished.  So a peer writing participation j + 1 (parity flipped) can overlap this
+// block's reads of participation j, but nothing writes parity j & 1 again until those reads are done.
+constexpr int kSyncT = 64;                       // threads of a sync block; a thread owns 4 channels
+constexpr int kSyncStep = kSyncT * 4;            // channels per block step
+constexpr int kMaxSyncBlocks = 8;
+constexpr int kSyncPad = 4 * kMaxSyncBlocks;     // floats of the count vectors at the head of a slot
+
+__device__ __forceinline__ Vec16 ld_vec4(const float* p) { return *reinterpret_cast<const Vec16*>(p); }
+__device__ __forceinline__ void unpack4(const Vec16& v, float* f) { TagF32::unpack(v, f); }
+
+// kStats: push (M_r, mean, M2), merge in rank order with Chan's formula and write mean, invstd, the running
+// statistics and the total count.  Otherwise: push (dbias, dweight) partials and write their rank-ordered sums.
+template <bool kStats>
+__global__ void __launch_bounds__(kSyncT) bn_sync_kernel(PeerView pv, int channel, size_t win_off, int cmax, int C,
+                                                         const float* __restrict__ a_in,
+                                                         const float* __restrict__ b_in, float count, float eps,
+                                                         float momentum, float* run_mean, float* run_var,
+                                                         float* out_a, float* out_b, float* total) {
+  const int W = pv.world, me = pv.rank;
+  const size_t slot = kSyncPad + 2 * (size_t)cmax;
+  const size_t par = pv.epoch[channel * kMaxBlocks + blockIdx.x] & 1u;
+  const size_t mine = (par * W + me) * slot;
+  for (int c = (blockIdx.x * kSyncT + threadIdx.x) * 4; c < C; c += gridDim.x * kSyncStep) {
+    const Vec16 va = ld_vec4(a_in + c), vb = ld_vec4(b_in + c);
+    for (int p = 0; p < W; ++p) {
+      float* dst = reinterpret_cast<float*>(pv.data[p] + win_off) + mine + kSyncPad;
+      st_peer16(dst + c, va);
+      st_peer16(dst + cmax + c, vb);
+    }
+  }
+  if (kStats && threadIdx.x < W) {
+    float* dst = reinterpret_cast<float*>(pv.data[threadIdx.x] + win_off) + mine + 4 * blockIdx.x;
+    st_peer16(dst, Vec16{__float_as_uint(count), 0u, 0u, 0u});
+  }
+  barrier_peers(pv, channel);
+
+  const float* win = reinterpret_cast<const float*>(pv.data[me] + win_off) + par * W * slot;
+  for (int c = (blockIdx.x * kSyncT + threadIdx.x) * 4; c < C; c += gridDim.x * kSyncStep) {
+    float n = 0.f, a[4] = {0.f, 0.f, 0.f, 0.f}, b[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int r = 0; r < W; ++r) {
+      const float* s = win + r * slot;
+      float ra[4], rb[4];
+      unpack4(ld_peer16(s + kSyncPad + c), ra);
+      unpack4(ld_peer16(s + kSyncPad + cmax + c), rb);
+      if constexpr (kStats) {
+        chan_merge<4>(n, a, b, __uint_as_float(ld_peer16(s + 4 * blockIdx.x).x), ra, rb);
+      } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          a[k] += ra[k];
+          b[k] += rb[k];
+        }
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if constexpr (kStats) {
+        out_a[c + k] = a[k];
+        out_b[c + k] = 1.f / sqrtf(b[k] / n + eps);
+        if (run_mean != nullptr) {
+          run_mean[c + k] = momentum * a[k] + (1.f - momentum) * run_mean[c + k];
+          run_var[c + k] = momentum * (b[k] / (n - 1.f)) + (1.f - momentum) * run_var[c + k];
+        }
+      } else {
+        out_a[c + k] = a[k];
+        out_b[c + k] = b[k];
+      }
+    }
+    if (kStats && c == 0) *total = n;
   }
 }
 
@@ -492,7 +587,7 @@ cudaError_t launch_bn_act_fwd_stats(const void* x, int dtype, size_t M, int C, f
   int G;
   chunks(M, g, &rpc, &G);
   const dim3 grid(G, g.ncb);
-  BN_DISPATCH_U(dtype, (bn_act_fwd_stats_kernel<U><<<grid, kT, 0, s>>>(x, M, C, g.shift, rpc, eps, momentum,
+  BN_DISPATCH_U(dtype, (bn_act_fwd_stats_kernel<U, false><<<grid, kT, 0, s>>>(x, M, C, g.shift, rpc, eps, momentum,
                                                                         running_mean, running_var, save_mean,
                                                                         save_invstd, ws, counters)));
   return cudaGetLastError();
@@ -528,15 +623,107 @@ cudaError_t launch_bn_act_bwd_reduce(const void* dy, const void* x, const uint8_
 
 cudaError_t launch_bn_act_bwd_apply(const void* dy, const void* x, const uint8_t* mask, int dtype, size_t M, int C,
                                     const float* mean, const float* invstd, const float* weight, const float* dweight,
-                                    const float* dbias, void* dx, void* dresidual, cudaStream_t s) {
+                                    const float* dbias, void* dx, void* dresidual, cudaStream_t s,
+                                    const float* total) {
   if (bad_shape(M, C) || !aligned16(dy) || !aligned16(x) || !aligned16(dx) || !aligned16(dresidual))
     return cudaErrorInvalidValue;
   const Geo g = geo(C, kMaxCB);
   const dim3 grid(apply_grid(M, g, kBwdApplyBlocksPerSM), g.ncb);
-  BN_DISPATCH_U(dtype, BN_DISPATCH_B(mask != nullptr, kRelu, BN_DISPATCH_B(dresidual != nullptr, kRes, (
-      bn_act_bwd_apply_kernel<U, kRelu, kRes><<<grid, kT, 0, s>>>(dy, x, mask, M, C, g.shift, mean, invstd, weight,
-                                                                  dweight, dbias, dx, dresidual)))));
+  BN_DISPATCH_U(dtype, BN_DISPATCH_B(mask != nullptr, kRelu, BN_DISPATCH_B(dresidual != nullptr, kRes,
+      BN_DISPATCH_B(total != nullptr, kTotal, (bn_act_bwd_apply_kernel<U, kRelu, kRes, kTotal><<<grid, kT, 0, s>>>(
+          dy, x, mask, M, C, g.shift, mean, invstd, weight, dweight, dbias, dx, dresidual, total))))));
   return cudaGetLastError();
+}
+
+cudaError_t launch_bn_act_fwd_stats_local(const void* x, int dtype, size_t M, int C, float* local_mean,
+                                          float* local_m2, float* ws, uint32_t* counters, cudaStream_t s) {
+  if (bad_shape(M, C) || !aligned16(x)) return cudaErrorInvalidValue;
+  const Geo g = geo(C, red_cb(C));
+  size_t rpc;
+  int G;
+  chunks(M, g, &rpc, &G);
+  const dim3 grid(G, g.ncb);
+  BN_DISPATCH_U(dtype, (bn_act_fwd_stats_kernel<U, true><<<grid, kT, 0, s>>>(x, M, C, g.shift, rpc, 0.f, 0.f,
+                                                                             nullptr, nullptr, local_mean, local_m2,
+                                                                             ws, counters)));
+  return cudaGetLastError();
+}
+
+size_t bn_sync_window_floats(int world, int cmax) { return 2 * (size_t)world * (kSyncPad + 2 * (size_t)cmax); }
+
+namespace {
+cudaError_t check_sync(const PeerView& pv, int channel, const void* window, int cmax, int C, const float* a,
+                       const float* b) {
+  if (pv.world < 1 || pv.world > kMaxRanks || channel < 0 || channel > 1 || C < kCh || C % kCh != 0 || C > cmax ||
+      cmax % kCh != 0 || !aligned16(window) || !aligned16(a) || !aligned16(b))
+    return cudaErrorInvalidValue;
+  return cudaSuccess;
+}
+int sync_grid(int C) {
+  const int steps = (C + kSyncStep - 1) / kSyncStep;
+  return steps < kMaxSyncBlocks ? steps : kMaxSyncBlocks;
+}
+}  // namespace
+
+cudaError_t launch_bn_sync_stats(const PeerView& pv, int channel, size_t win_off, int cmax, int C,
+                                 const float* local_mean, const float* local_m2, float count, float eps,
+                                 float momentum, float* running_mean, float* running_var, float* save_mean,
+                                 float* save_invstd, float* total, cudaStream_t s) {
+  if (check_sync(pv, channel, pv.data[pv.rank] + win_off, cmax, C, local_mean, local_m2) != cudaSuccess ||
+      !(count >= 1.f) || (running_mean == nullptr) != (running_var == nullptr) || total == nullptr)
+    return cudaErrorInvalidValue;
+  bn_sync_kernel<true><<<sync_grid(C), kSyncT, 0, s>>>(pv, channel, win_off, cmax, C, local_mean, local_m2, count,
+                                                       eps, momentum, running_mean, running_var, save_mean,
+                                                       save_invstd, total);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_bn_sync_grad(const PeerView& pv, int channel, size_t win_off, int cmax, int C, const float* dbias,
+                                const float* dweight, float* sum_dbias, float* sum_dweight, cudaStream_t s) {
+  if (check_sync(pv, channel, pv.data[pv.rank] + win_off, cmax, C, dbias, dweight) != cudaSuccess)
+    return cudaErrorInvalidValue;
+  bn_sync_kernel<false><<<sync_grid(C), kSyncT, 0, s>>>(pv, channel, win_off, cmax, C, dbias, dweight, 0.f, 0.f,
+                                                        0.f, nullptr, nullptr, sum_dbias, sum_dweight, nullptr);
+  return cudaGetLastError();
+}
+
+namespace {
+template <class K>
+cudaError_t load1(K* kernel) {
+  cudaFuncAttributes a;
+  return cudaFuncGetAttributes(&a, (const void*)kernel);
+}
+template <class U>
+cudaError_t load_u() {
+  cudaError_t e = cudaSuccess;
+  auto keep = [&e](cudaError_t x) { if (e == cudaSuccess) e = x; };
+  keep(load1(bn_act_fwd_stats_kernel<U, false>));
+  keep(load1(bn_act_fwd_stats_kernel<U, true>));
+  keep(load1(bn_act_fwd_apply_kernel<U, false, false>));
+  keep(load1(bn_act_fwd_apply_kernel<U, false, true>));
+  keep(load1(bn_act_fwd_apply_kernel<U, true, false>));
+  keep(load1(bn_act_fwd_apply_kernel<U, true, true>));
+  keep(load1(bn_act_bwd_reduce_kernel<U, false>));
+  keep(load1(bn_act_bwd_reduce_kernel<U, true>));
+  keep(load1(bn_act_bwd_apply_kernel<U, false, false, false>));
+  keep(load1(bn_act_bwd_apply_kernel<U, false, true, false>));
+  keep(load1(bn_act_bwd_apply_kernel<U, true, false, false>));
+  keep(load1(bn_act_bwd_apply_kernel<U, true, true, false>));
+  keep(load1(bn_act_bwd_apply_kernel<U, false, false, true>));
+  keep(load1(bn_act_bwd_apply_kernel<U, false, true, true>));
+  keep(load1(bn_act_bwd_apply_kernel<U, true, false, true>));
+  keep(load1(bn_act_bwd_apply_kernel<U, true, true, true>));
+  return e;
+}
+}  // namespace
+
+cudaError_t bn_act_load_kernels() {
+  cudaError_t e = load_u<TagF32>();
+  if (e == cudaSuccess) e = load_u<TagBF16>();
+  if (e == cudaSuccess) e = load_u<TagF16>();
+  if (e == cudaSuccess) e = load1(bn_sync_kernel<true>);
+  if (e == cudaSuccess) e = load1(bn_sync_kernel<false>);
+  return e;
 }
 
 }  // namespace bps

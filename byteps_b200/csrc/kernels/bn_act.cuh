@@ -20,6 +20,8 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include "kernels/peer_view.h"
+
 namespace bps {
 
 size_t bn_act_workspace_floats(size_t M, int C);
@@ -34,8 +36,37 @@ cudaError_t launch_bn_act_fwd_apply(const void* x, const void* residual, int dty
 cudaError_t launch_bn_act_bwd_reduce(const void* dy, const void* x, const uint8_t* mask, int dtype, size_t M, int C,
                                      const float* mean, const float* invstd, float* dweight, float* dbias, float* ws,
                                      uint32_t* counters, cudaStream_t s);
+// total: device pointer to the row count the statistics were formed over (synchronised batch norm: all ranks'
+// rows, written by launch_bn_sync_stats); nullptr divides by M.
 cudaError_t launch_bn_act_bwd_apply(const void* dy, const void* x, const uint8_t* mask, int dtype, size_t M, int C,
                                     const float* mean, const float* invstd, const float* weight, const float* dweight,
-                                    const float* dbias, void* dx, void* dresidual, cudaStream_t s);
+                                    const float* dbias, void* dx, void* dresidual, cudaStream_t s,
+                                    const float* total = nullptr);
+
+// ---- synchronised batch norm (torch.nn.SyncBatchNorm semantics) over peer-mapped memory --------------------
+//
+//   fwd_stats_local   fwd_stats in local-partials mode: this rank's per-channel mean and M2 over its M >= 1 rows
+//   sync_stats        pushes (M_r, mean, M2) into every peer's window, meets the peers (barrier_peers on
+//                     `channel`), merges the W partials in rank order with Chan's formula; writes mean, invstd
+//                     (biased variance), the running statistics (unbiased variance) and the total count N.  Every
+//                     rank performs the same operations in the same order, so all ranks get the same bits.  N must
+//                     be at least 2.
+//   sync_grad         the same exchange for bwd_reduce's local (dbias, dweight) = (sum g, invstd * sum g (x - mean));
+//                     writes their sums over the ranks in rank order, which bwd_apply reads together with N.
+//
+// The window at pv.data[r] + win_off holds bn_sync_window_floats(world, cmax) floats (16-byte aligned) on every
+// rank; C <= cmax.  Launches on one rank must come from one stream, in the same order on every
+// rank, and every kernel a rank may launch must be loaded (bn_act_load_kernels) before the first one, since a
+// module load while a peer's kernel spins can deadlock.  The grids are at most 8 blocks of 64 threads.
+size_t bn_sync_window_floats(int world, int cmax);
+cudaError_t bn_act_load_kernels();
+cudaError_t launch_bn_act_fwd_stats_local(const void* x, int dtype, size_t M, int C, float* local_mean,
+                                          float* local_m2, float* ws, uint32_t* counters, cudaStream_t s);
+cudaError_t launch_bn_sync_stats(const PeerView& pv, int channel, size_t win_off, int cmax, int C,
+                                 const float* local_mean, const float* local_m2, float count, float eps,
+                                 float momentum, float* running_mean, float* running_var, float* save_mean,
+                                 float* save_invstd, float* total, cudaStream_t s);
+cudaError_t launch_bn_sync_grad(const PeerView& pv, int channel, size_t win_off, int cmax, int C, const float* dbias,
+                                const float* dweight, float* sum_dbias, float* sum_dweight, cudaStream_t s);
 
 }  // namespace bps

@@ -95,6 +95,10 @@ class BatchNormAct2d(nn.BatchNorm2d):
                 and x.numel() > x.size(1)
                 and (residual is None or (residual.shape == x.shape and residual.dtype == x.dtype and _nhwc(residual))))
 
+    def _fused(self, x, residual, running_mean, running_var, factor):
+        return _BatchNormActFn.apply(x, residual, self.weight, self.bias, running_mean, running_var, factor, self.eps,
+                                     self.act == "relu")
+
     def forward(self, x, residual=None):
         # statistics bookkeeping exactly as nn.BatchNorm2d.forward
         self._check_input_dim(x)
@@ -107,11 +111,205 @@ class BatchNormAct2d(nn.BatchNorm2d):
         running_mean = self.running_mean if track else None
         running_var = self.running_var if track else None
         if self._fusable(x, residual, batch_stats):
-            return _BatchNormActFn.apply(x, residual, self.weight, self.bias, running_mean, running_var, factor,
-                                         self.eps, self.act == "relu")
+            return self._fused(x, residual, running_mean, running_var, factor)
         y = F.batch_norm(x, running_mean, running_var, self.weight, self.bias, batch_stats, factor, self.eps)
         if residual is not None:
             y = y + residual
         if self.act == "relu":
             y = F.relu(y, inplace=True)
         return y
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Synchronised batch norm: statistics and gradient sums over the union of all ranks' batches
+# (torch.nn.SyncBatchNorm semantics), exchanged through a peer-mapped window by two small kernels.
+
+class SyncBatchNormContext:
+    """Cross-rank state shared by every synchronised batch norm of a model on one rank.
+
+    It owns (or borrows, for a :class:`~byteps_b200.comm.symm.VirtualCluster` rank) a peer-mapped window of
+    ``[parity][source rank][count vectors + 2 * cmax]`` floats and the barrier generations of its own signal pad,
+    separate from the exchange's arena, so the sync kernels never interfere with the exchange kernels running on
+    the communication stream.  The sync kernels of every layer meet the peers in the same order on every rank, so
+    all calls on one rank must come from one CUDA stream, in program order; a call from another stream raises.
+    """
+
+    channel = 0   # barrier channel of the context's own signal pad
+
+    def __init__(self, view, rank: int, world: int, cmax: int, owner=None, stream: Optional[int] = None):
+        self.view, self.rank, self.world, self.cmax = view, rank, world, cmax
+        self._owner = owner      # keeps the peer-mapped memory alive
+        self._stream = stream
+        # Every kernel variant a rank may launch is loaded now: CUDA loading a module lazily while a peer's sync
+        # kernel spins on this rank can deadlock.
+        _native.cuda().bn_act_load_kernels()
+
+    @staticmethod
+    def window_bytes(world: int, cmax: int) -> int:
+        return 4 * int(_native.cuda().bn_sync_window_floats(world, cmax))
+
+    @classmethod
+    def create(cls, group, device, cmax: int, mode: str = "auto") -> "SyncBatchNormContext":
+        """Collective: a dedicated symmetric-memory context for ``group`` (every rank must call it)."""
+        from ..comm.symm import SymmContext
+
+        cmax = max(_UNIT, -(-int(cmax) // _UNIT) * _UNIT)
+        symm = SymmContext(group, device, cls.window_bytes(group.world, cmax), mode, "0")
+        return cls(symm.view, symm.rank, symm.world, cmax, owner=symm)
+
+    @classmethod
+    def from_virtual(cls, cluster, rank: int, cmax: int) -> "SyncBatchNormContext":
+        """Rank ``rank`` of a VirtualCluster (window at offset 0 of its arena), bound to that rank's stream."""
+        cmax = max(_UNIT, -(-int(cmax) // _UNIT) * _UNIT)
+        if cls.window_bytes(cluster.world, cmax) > cluster.data_bytes:
+            raise ValueError("VirtualCluster arena of %d bytes is smaller than the %d-byte window" % (
+                cluster.data_bytes, cls.window_bytes(cluster.world, cmax)))
+        return cls(cluster.views[rank], rank, cluster.world, cmax, owner=cluster,
+                   stream=cluster.streams[rank].cuda_stream)
+
+    def stream_for(self, device) -> int:
+        s = torch.cuda.current_stream(device).cuda_stream
+        if self._stream is None:
+            self._stream = s
+        elif s != self._stream:
+            raise RuntimeError("synchronised batch norm: rank %d was called on stream 0x%x, but its earlier calls used "
+                               "0x%x; every call on a rank must come from one stream" % (self.rank, s, self._stream))
+        return s
+
+    def __deepcopy__(self, memo):
+        return self   # peer-mapped memory is not copied: a deep-copied model keeps its ranks' window
+
+
+class _SyncBatchNormActFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, residual, weight, bias, running_mean, running_var, momentum, eps, relu, sync):
+        cu = _native.cuda()
+        n, c, h, w = x.shape
+        m = n * h * w
+        code = _CODES[x.dtype]
+        stream = sync.stream_for(x.device)
+        f32 = dict(dtype=torch.float32, device=x.device)
+        local = torch.empty(2, c, **f32)               # this rank's mean, M2
+        mean, invstd = torch.empty(c, **f32), torch.empty(c, **f32)
+        total = torch.empty(1, **f32)                  # row count of all ranks
+        nws, nctr = cu.bn_act_workspace(m, c)
+        ws = torch.empty(nws, **f32)
+        ctr = torch.zeros(nctr, dtype=torch.int32, device=x.device)
+        cu.bn_act_fwd_stats_local(x.data_ptr(), code, m, c, local[0].data_ptr(), local[1].data_ptr(), ws.data_ptr(),
+                                  ctr.data_ptr(), stream)
+        cu.bn_sync_stats(sync.view, sync.channel, 0, sync.cmax, c, local[0].data_ptr(), local[1].data_ptr(), float(m),
+                         float(eps), float(momentum), _ptr(running_mean), _ptr(running_var), mean.data_ptr(),
+                         invstd.data_ptr(), total.data_ptr(), stream)
+        y = torch.empty_like(x)
+        mask = torch.empty((m, c // _UNIT), dtype=torch.uint8, device=x.device) if relu else None
+        cu.bn_act_fwd_apply(x.data_ptr(), _ptr(residual), code, m, c, mean.data_ptr(), invstd.data_ptr(),
+                            weight.data_ptr(), bias.data_ptr(), bool(relu), y.data_ptr(), _ptr(mask), stream)
+        ctx.save_for_backward(x, weight, mean, invstd, mask, total)
+        ctx.has_residual = residual is not None
+        ctx.sync = sync
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, weight, mean, invstd, mask, total = ctx.saved_tensors
+        sync = ctx.sync
+        cu = _native.cuda()
+        n, c, h, w = x.shape
+        m = n * h * w
+        code = _CODES[x.dtype]
+        dy = dy.to(x.dtype).contiguous(memory_format=torch.channels_last)
+        stream = sync.stream_for(x.device)
+        f32 = dict(dtype=torch.float32, device=x.device)
+        dweight, dbias = torch.empty(c, **f32), torch.empty(c, **f32)
+        nws, nctr = cu.bn_act_workspace(m, c)
+        ws = torch.empty(nws, **f32)
+        ctr = torch.zeros(nctr, dtype=torch.int32, device=x.device)
+        cu.bn_act_bwd_reduce(dy.data_ptr(), x.data_ptr(), _ptr(mask), code, m, c, mean.data_ptr(), invstd.data_ptr(),
+                             dweight.data_ptr(), dbias.data_ptr(), ws.data_ptr(), ctr.data_ptr(), stream)
+        sums = torch.empty(2, c, **f32)                # sum over ranks of dbias, dweight
+        cu.bn_sync_grad(sync.view, sync.channel, 0, sync.cmax, c, dbias.data_ptr(), dweight.data_ptr(),
+                        sums[0].data_ptr(), sums[1].data_ptr(), stream)
+        dx = torch.empty_like(x)
+        dres = torch.empty_like(x) if ctx.has_residual else None
+        cu.bn_act_bwd_apply(dy.data_ptr(), x.data_ptr(), _ptr(mask), code, m, c, mean.data_ptr(), invstd.data_ptr(),
+                            weight.data_ptr(), sums[1].data_ptr(), sums[0].data_ptr(), dx.data_ptr(), _ptr(dres),
+                            stream, total.data_ptr())
+        # the local sums, as torch.nn.SyncBatchNorm: the gradient exchange averages them over the ranks
+        return dx, dres, dweight, dbias, None, None, None, None, None, None
+
+
+class SyncBatchNormAct2d(BatchNormAct2d):
+    """:class:`BatchNormAct2d` whose training-mode statistics are those of all ranks' batches together.
+
+    Forward normalises with the mean and biased variance of the union of the ranks' batches (ranks may hold
+    different row counts); the running statistics take the global unbiased variance and are bit-identical on every
+    rank.  Backward forms dx from the all-reduced sums and returns the rank's local dweight / dbias.  Training at
+    world > 1 needs a fusable input (CUDA, channels_last, C a multiple of 8, fp32/bf16/fp16 activations, fp32
+    affine parameters) and raises ``ValueError`` otherwise; eval mode and world 1 are :class:`BatchNormAct2d`.
+    """
+
+    def __init__(self, num_features, eps=1e-5, momentum=0.1, affine=True, track_running_stats=True, act=None,
+                 sync: Optional[SyncBatchNormContext] = None, device=None, dtype=None):
+        super().__init__(num_features, eps, momentum, affine, track_running_stats, act, device, dtype)
+        self.sync = sync
+
+    def _synced(self):
+        return self.training and self.sync is not None and self.sync.world > 1
+
+    def _unfusable(self, x, residual) -> Optional[str]:
+        """Why a training input cannot take the synchronised kernels, or None."""
+        if not x.is_cuda:
+            return "the input is not a CUDA tensor"
+        if x.dtype not in _CODES:
+            return "the input dtype %s is not float32, bfloat16 or float16" % x.dtype
+        if not self.affine or self.weight.dtype != torch.float32:
+            return "the affine parameters must exist and be float32"
+        if x.size(1) % _UNIT != 0:
+            return "C = %d is not a multiple of %d" % (x.size(1), _UNIT)
+        if x.size(1) > self.sync.cmax:
+            return "C = %d exceeds the context's %d channels" % (x.size(1), self.sync.cmax)
+        if x.numel() == 0:
+            return "the input is empty"
+        if not _nhwc(x):
+            return "the input is not channels_last (NHWC) contiguous"
+        if residual is not None and not (residual.shape == x.shape and residual.dtype == x.dtype and _nhwc(residual)):
+            return "the residual does not match the input's shape, dtype and channels_last layout"
+        return None
+
+    def _fusable(self, x, residual, batch_stats):
+        return True if self._synced() else super()._fusable(x, residual, batch_stats)
+
+    def _fused(self, x, residual, running_mean, running_var, factor):
+        if not self._synced():
+            return super()._fused(x, residual, running_mean, running_var, factor)
+        return _SyncBatchNormActFn.apply(x, residual, self.weight, self.bias, running_mean, running_var, factor,
+                                         self.eps, self.act == "relu", self.sync)
+
+    def forward(self, x, residual=None):
+        if self._synced():
+            self._check_input_dim(x)
+            why = self._unfusable(x, residual)
+            if why is not None:
+                raise ValueError("SyncBatchNormAct2d: synchronised training needs a fusable input, but %s" % why)
+        return super().forward(x, residual)
+
+
+def convert_sync_batchnorm(module: nn.Module, sync: Optional[SyncBatchNormContext]) -> nn.Module:
+    """Replace every ``nn.BatchNorm2d`` in ``module`` (``BatchNormAct2d`` included, keeping its ``act``) by a
+    :class:`SyncBatchNormAct2d` on ``sync`` that holds the same Parameter and buffer objects, so optimizers built
+    over the original parameters stay valid and state_dict keys and parameter order are unchanged.  Children are
+    replaced in place; the converted module is returned."""
+    if isinstance(module, nn.BatchNorm2d):
+        new = SyncBatchNormAct2d(module.num_features, module.eps, module.momentum, module.affine,
+                                 module.track_running_stats, act=getattr(module, "act", None), sync=sync,
+                                 device="meta")
+        new.weight, new.bias = module.weight, module.bias
+        new.running_mean, new.running_var = module.running_mean, module.running_var
+        new.num_batches_tracked = module.num_batches_tracked
+        new.train(module.training)
+        if hasattr(module, "qconfig"):
+            new.qconfig = module.qconfig
+        return new
+    for name, child in module.named_children():
+        module.add_module(name, convert_sync_batchnorm(child, sync))
+    return module

@@ -35,7 +35,7 @@ __all__ = [
     "init", "shutdown", "suspend", "resume", "rank", "size", "local_rank", "local_size", "get_pushpull_speed",
     "push_pull", "push_pull_async", "push_pull_inplace", "push_pull_async_inplace", "push_pull_group_sync_inplace",
     "poll", "synchronize", "declare", "byteps_torch_set_num_grads", "DistributedOptimizer", "broadcast_parameters",
-    "broadcast_optimizer_state", "broadcast_object", "Compression", "set_learning_rate",
+    "broadcast_optimizer_state", "broadcast_object", "Compression", "set_learning_rate", "convert_sync_batchnorm",
 ]
 
 
@@ -540,3 +540,26 @@ def broadcast_object(obj, root_rank=0, name=None):
     if rank() != root_rank:
         obj = cloudpickle.load(io.BytesIO(t.numpy().tobytes()))
     return obj
+
+
+def convert_sync_batchnorm(module):
+    """Synchronised batch norm: the counterpart of ``torch.nn.SyncBatchNorm.convert_sync_batchnorm``.
+
+    Replaces every ``nn.BatchNorm2d`` of ``module`` (the models' ``BatchNormAct2d`` included, keeping their
+    activation and residual input) by :class:`~byteps_b200.ops.bn_act.SyncBatchNormAct2d`, which normalises with
+    the statistics of all ranks' batches in training.  The new modules hold the same Parameter and buffer objects,
+    so a ``DistributedOptimizer`` built before or after the call stays valid.  Call it after ``init()``; it is
+    collective (every rank calls it on the same model) and needs the symmetric-memory backend.  Returns the
+    converted module."""
+    from ..ops.bn_act import SyncBatchNormContext
+    from ..ops.bn_act import convert_sync_batchnorm as _convert
+
+    eng = _engine()
+    if eng.backend not in ("local", "symm"):
+        raise ValueError("convert_sync_batchnorm needs the symmetric-memory backend; this job uses %r" % eng.backend)
+    sync = None
+    if eng.size > 1:
+        cmax = max([m.num_features for m in module.modules() if isinstance(m, torch.nn.BatchNorm2d)] or [8])
+        sync = SyncBatchNormContext.create(eng.group, torch.device("cuda", torch.cuda.current_device()), cmax,
+                                           eng.cfg.symm_mode)
+    return _convert(module, sync)

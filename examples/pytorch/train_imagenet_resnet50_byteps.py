@@ -32,6 +32,8 @@ p.add_argument("--model", default="resnet50")
 p.add_argument("--image-size", type=int, default=224)
 p.add_argument("--no-cuda", action="store_true")
 p.add_argument("--fused-update", action="store_true", help="SGD step inside the exchange kernel (fp32 master shards)")
+p.add_argument("--sync-bn", action="store_true",
+               help="batch-norm statistics over all ranks' batches (bps.convert_sync_batchnorm; CUDA channels_last)")
 args = p.parse_args()
 bps.init()
 cuda = torch.cuda.is_available() and not args.no_cuda
@@ -45,6 +47,9 @@ for e in range(args.epochs, 0, -1):
         break
 resume_from = int(bps.broadcast_object(resume_from, 0, name="resume_from_epoch"))
 model = get_model(args.model).to(dev)
+if args.sync_bn:
+    # synchronised training takes NHWC (channels_last) activations; converting is collective
+    model = bps.convert_sync_batchnorm(model.to(memory_format=torch.channels_last))
 opt = torch.optim.SGD(model.parameters(), lr=args.base_lr * args.batches_per_pushpull * bps.size(), momentum=0.9,
                       weight_decay=5e-5)
 opt = bps.DistributedOptimizer(opt, named_parameters=model.named_parameters(),
@@ -65,6 +70,8 @@ for epoch in range(resume_from, args.epochs):
         opt.zero_grad()
         for _ in range(args.batches_per_pushpull):
             x = torch.rand(args.batch_size, 3, args.image_size, args.image_size, device=dev)
+            if args.sync_bn:
+                x = x.contiguous(memory_format=torch.channels_last)
             y = torch.randint(0, 1000, (args.batch_size,), device=dev)
             loss = F.cross_entropy(model(x), y) / args.batches_per_pushpull
             loss.backward()
