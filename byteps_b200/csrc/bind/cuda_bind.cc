@@ -10,6 +10,7 @@
 
 #include "bind/cuda_bind_ext.h"
 #include "comm/symm_mem.h"
+#include "kernels/loss_scale.cuh"
 #include "kernels/pushpull.cuh"
 
 namespace py = pybind11;
@@ -205,6 +206,34 @@ PYBIND11_MODULE(_cuda, m) {
         check(launch_barrier(pv, blocks, channel, (cudaStream_t)stream), "barrier");
       },
       py::arg("view"), py::arg("blocks") = 1, py::arg("channel") = 0, py::arg("stream") = 0);
+
+  // ---- dynamic loss scaling of the fused optimizer (kernels/loss_scale.cu)
+  m.attr("LOSS_SCALE_ENTRY_BYTES") = (int)sizeof(LossScaleCheckEntry);
+  m.attr("LOSS_SCALE_STATE_BYTES") = (int)sizeof(LossScaleState);
+  m.attr("LOSS_SCALE_WINDOW_BYTES") = kLossScaleWindowBytes;
+  m.def(
+      "loss_scale_check",
+      [](const PeerView& pv, uintptr_t table, int nentries, size_t max_vectors, uintptr_t state, uintptr_t stream) {
+        check(launch_loss_scale_check(pv, (const LossScaleCheckEntry*)table, nentries, max_vectors,
+                                      (LossScaleState*)state, (cudaStream_t)stream),
+              "loss_scale_check");
+      },
+      py::arg("view"), py::arg("table"), py::arg("nentries"), py::arg("max_vectors"), py::arg("state"),
+      py::arg("stream") = 0, "OR an overflow flag of this rank's gradient windows into state.found");
+  m.def(
+      "loss_scale_update",
+      [](const PeerView& pv, int channel, size_t win_off, uintptr_t state, uintptr_t steps, uintptr_t betas,
+         uintptr_t hp, int ngroups, bool adam, uintptr_t stream) {
+        check(launch_loss_scale_update(pv, channel, win_off, (LossScaleState*)state, (int32_t*)steps,
+                                       (const double*)betas, (OptHParams*)hp, ngroups, adam ? 1 : 0,
+                                       (cudaStream_t)stream),
+              "loss_scale_update");
+      },
+      py::arg("view"), py::arg("channel"), py::arg("win_off"), py::arg("state"), py::arg("steps"), py::arg("betas"),
+      py::arg("hp"), py::arg("ngroups"), py::arg("adam"), py::arg("stream") = 0,
+      "agree on the overflow flag with every peer, update the scale and write the step's hyper-parameters");
+  m.def("loss_scale_load_kernels", []() { check(loss_scale_load_kernels(), "loss_scale_load_kernels"); },
+        "load the loss-scaling kernels now (before any cross-rank launch)");
 
   m.def("shard_units", [](size_t total_units, int world, int rank) {
     size_t b, e;

@@ -111,6 +111,7 @@ __global__ void __launch_bounds__(512) pushpull_fused_opt_kernel(PeerView pv, co
   Epi epi = epi_proto;
   epi.shard_begin = s0 * E;
   epi.hp = *hp;
+  if (epi.hp.skip) s1 = s0;     // a step skipped by dynamic loss scaling: no update, nothing written
   reduce_phase<W, kUnrollOpt>(pv, stage_off, s0, s1, nvls != 0, rot_of(pv), epi,
                            [&](const float* f, size_t unit) { sink_peers<P, E>(pv, param_off, unit, f, nvls != 0); });
   barrier_peers(pv, channel);
@@ -170,6 +171,7 @@ __global__ void __launch_bounds__(kOptThreads, 2) pushpull_fused_opt_tma_kernel(
   Epi epi = epi_proto;
   epi.shard_begin = s0 * E;
   epi.hp = *hp;
+  if (epi.hp.skip) s1 = s0;     // a step skipped by dynamic loss scaling: no tile, nothing written
   const int nstreams = epi.active_streams();
   const bool is_producer = (threadIdx.x >> 5) == (kOptTileUnits >> 5);
 

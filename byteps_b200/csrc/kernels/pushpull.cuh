@@ -46,7 +46,8 @@ struct OptHParams {
   int adamw;         // decoupled weight decay
   int first_step;    // momentum buffer initialisation (buf = g)
   float grad_scale;  // extra multiplier on the reduced gradient (loss-scale^-1)
-  int pad[3];
+  int skip;          // dynamic loss scaling found an overflow: leave the optimizer state as it is
+  int pad[2];
 };
 
 struct LaunchCfg {

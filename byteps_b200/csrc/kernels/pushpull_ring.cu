@@ -105,6 +105,9 @@ __device__ __forceinline__ void process_desc(const PeerView& pv, const RingDesc&
   constexpr int E = W::kPerVec;
   size_t s0, s1;
   shard_units_of<E>(d.groups, pv.world, pv.rank, &s0, &s1);
+  if constexpr (KIND != RING_ALLREDUCE) {
+    if (d.hp->skip) return;     // a step skipped by dynamic loss scaling: no update, nothing written
+  }
   const int rot = rot_of(pv);
   const size_t goff = d.grad_off, poff = d.param_off;
   if constexpr (KIND == RING_ALLREDUCE) {

@@ -128,6 +128,8 @@ def resync_fused_masters():
 
 
 _HP_FMT = "<9f3if3i"   # matches csrc/kernels/pushpull.cuh::OptHParams (64 bytes)
+_LS_STATE_FMT = "<2df5i"   # csrc/kernels/loss_scale.cuh::LossScaleState (40 bytes)
+_LS_ENTRY_FMT = "<2Q4i"    # csrc/kernels/loss_scale.cuh::LossScaleCheckEntry (32 bytes)
 
 
 class BucketedGradSync:
@@ -135,10 +137,15 @@ class BucketedGradSync:
 
     def __init__(self, engine, param_groups, *, fused: Optional[str] = None, wire_dtype: Optional[torch.dtype] = None,
                  bucket_bytes: Optional[int] = None, backward_passes_per_step: int = 1, average: bool = True,
-                 priority_of: Optional[Dict] = None):
+                 priority_of: Optional[Dict] = None, loss_scaler: Optional[Dict] = None):
+        """loss_scaler (fused mode only): dynamic loss scaling on the device, a dict with GradScaler's
+        init_scale, growth_factor, backoff_factor and growth_interval (see `_issue_scaled_step`)."""
         self.engine = engine
         self.world, self.rank = engine.size, engine.rank
         self.fused = fused                     # None | "sgd" | "adam" | "adamw"
+        if loss_scaler is not None and not fused:
+            raise ValueError("dynamic loss scaling needs the fused optimizer")
+        self.loss_scaler = dict(loss_scaler) if loss_scaler is not None else None
         reduce_engine = os.environ.get("BYTEPS_REDUCE_ENGINE", "auto").lower()
         if reduce_engine not in REDUCE_ENGINES:
             raise ValueError("BYTEPS_REDUCE_ENGINE=%s: expected one of %s (the tensor-core engine of sm_90a is 'wgmma')"
@@ -185,6 +192,11 @@ class BucketedGradSync:
         if self._needs_stage():
             self.stage_bytes = max(self._wire_bytes(b) for b in self.buckets)
             off += (self.stage_bytes + 255) // 256 * 256
+        self.ls_win_off = -1
+        if self.loss_scaler is not None:
+            # the overflow flags every rank publishes to every peer (loss_scale_update), only in this mode
+            self.ls_win_off = off
+            off += 256
         cfg = engine.cfg
         stamp("buckets: layout of %d buckets, arena %d MiB" % (len(self.buckets), off >> 20))
         self.ctx = SymmContext(engine.group, self.device, max(off, 4096), cfg.symm_mode, cfg.use_nvls)
@@ -215,6 +227,8 @@ class BucketedGradSync:
             b.pending = len(b.params)
         if fused:
             self._init_fused_state()
+        if self.loss_scaler is not None:
+            self._init_loss_scaler()
         self._next = 0          # strict mode: next bucket index allowed to launch
         self._strict = os.environ.get("BYTEPS_STRICT_ORDER", "0") not in ("0", "")
         self._hooks = []
@@ -284,8 +298,61 @@ class BucketedGradSync:
             b.state1 = torch.zeros(n, dtype=torch.float32, device=self.device) if kind != "sgd" else None
         ng = len(self.param_groups)
         self._hp_dev = torch.zeros((ng, 64), dtype=torch.uint8, device=self.device)
-        self._group_step = [0] * ng
+        self._group_step = [0] * ng      # steps run (with dynamic loss scaling: attempted, skipped ones included)
         self.loss_scale = 1.0
+
+    # ------------------------------------------------------------------ dynamic loss scaling (fused mode)
+    def _init_loss_scaler(self):
+        """Device state of dynamic loss scaling: the scaler (LossScaleState), the applied-step count of every param
+        group, the float64 Adam betas the device forms the bias corrections from, and the check table, one entry
+        (gradient window, length, gradient dtype, wire dtype) per bucket."""
+        cu = self.ctx.cu
+        cu.loss_scale_load_kernels()     # loaded before any launch that spins on a peer (DESIGN 1.6)
+        ng = len(self.param_groups)
+        self._ls_state = torch.zeros(cu.LOSS_SCALE_STATE_BYTES, dtype=torch.uint8, device=self.device)
+        self._ls_steps = torch.zeros(ng, dtype=torch.int32, device=self.device)
+        self._ls_betas = torch.zeros((ng, 2), dtype=torch.float64, device=self.device)
+        blob = b"".join(struct.pack(_LS_ENTRY_FMT, b.grad_off, b.numel, wire_code(b.dtype), wire_code(self._wire(b)),
+                                    0, 0) for b in self.buckets)
+        self._ls_table = torch.frombuffer(bytearray(blob), dtype=torch.uint8).to(self.device)
+        self._ls_max_vectors = max(b.nbytes // 16 for b in self.buckets)
+        self.ctx.tensor(self.ls_win_off, 256, torch.uint8).zero_()
+        self.reset_loss_scaler()
+
+    def reset_loss_scaler(self):
+        """Scaler back to its initial values: scale = init_scale, growth tracker and skipped count 0."""
+        c = self.loss_scaler
+        self.set_loss_scaler_state(c["init_scale"], c["growth_factor"], c["backoff_factor"], c["growth_interval"], 0,
+                                   skipped=0)
+
+    def set_loss_scaler_state(self, scale, growth_factor, backoff_factor, growth_interval, growth_tracker,
+                              skipped=None):
+        """Install a scaler state (GradScaler.state_dict()'s values); skipped=None keeps the skipped count."""
+        if skipped is None:
+            skipped = self.loss_scaler_state()["skipped"]
+        vals = (float(growth_factor), float(backoff_factor), float(scale), int(growth_interval), int(growth_tracker),
+                int(skipped), 0, 0)
+        self._ls_state.copy_(torch.frombuffer(bytearray(struct.pack(_LS_STATE_FMT, *vals)), dtype=torch.uint8))
+
+    def loss_scaler_state(self) -> Dict:
+        """The scaler as the device holds it: scale, growth_factor, backoff_factor, growth_interval, tracker,
+        skipped, and steps (applied steps per group).  Synchronises with the current stream, which every step's
+        synchronize() has made wait for the exchanges."""
+        raw = self._ls_state.cpu().numpy().tobytes()
+        growth, backoff, scale, interval, tracker, skipped, _, _ = struct.unpack(_LS_STATE_FMT, raw)
+        return {"scale": scale, "growth_factor": growth, "backoff_factor": backoff, "growth_interval": interval,
+                "tracker": tracker, "skipped": skipped, "steps": self._ls_steps.tolist()}
+
+    def scale_tensor(self) -> torch.Tensor:
+        """0-dim float32 view of the device scale S (what the coming step's loss is multiplied by)."""
+        return self._ls_state[16:20].view(torch.float32)[0]
+
+    def applied_steps(self) -> List[int]:
+        """Steps the optimizer has applied per param group: with dynamic loss scaling the device's count (skipped
+        steps excluded; synchronises), otherwise the steps run."""
+        if self.loss_scaler is not None:
+            return self._ls_steps.tolist()
+        return list(self._group_step)
 
     def sync_master_from_params(self):
         for b in self.buckets:
@@ -336,6 +403,11 @@ class BucketedGradSync:
             blob += struct.pack(_HP_FMT, *vals)
         self.ctx.cu.write_blob(self._hp_dev.data_ptr(), blob, cur.cuda_stream)
         self.engine.launches += 1
+        if self.loss_scaler is not None and self.fused != "sgd":
+            # loss_scale_update forms Adam's bias corrections on the device, from the betas as the host holds them
+            betas = b"".join(struct.pack("<2d", *map(float, g.get("betas", (0.9, 0.999)))) for g in self.param_groups)
+            self.ctx.cu.write_blob(self._ls_betas.data_ptr(), betas, cur.cuda_stream)
+            self.engine.launches += 1
 
     # ------------------------------------------------------------------ hooks
     def _register_hooks(self):
@@ -362,7 +434,7 @@ class BucketedGradSync:
                 p.grad = gv
             b = self._param_bucket[p]
             b.pending -= 1
-            if b.pending == 0:
+            if b.pending == 0 and self.loss_scaler is None:   # dynamic loss scaling: launched at the step
                 self._launch_ready(b)
         return hook
 
@@ -395,6 +467,12 @@ class BucketedGradSync:
         else:
             self._ring_enqueue(b)
 
+    def _nvls_for(self, wire: torch.dtype) -> bool:
+        """Whether exchanges on this wire dtype use the in-switch (NVLS) reduction.  Not for an fp16 wire under dynamic
+        loss scaling: multimem.ld_reduce returns the rank sum in fp16, where values the overflow check passed can add
+        up to inf; the peer-load path sums them in fp32 registers instead (see loss_scale.cuh)."""
+        return bool(self.ctx.nvls) and not (self.loss_scaler is not None and wire == torch.float16)
+
     def _seg_table(self, b: Bucket) -> torch.Tensor:
         t = self._seg_tables.get(b.index)
         if t is None:
@@ -423,7 +501,7 @@ class BucketedGradSync:
         wbytes = self._wire_bytes(b)
         shard = (wbytes + world - 1) // world
         blocks = self.engine.cfg.comm_blocks or pick_blocks(shard, self.threads, 32, cap=64)
-        nvls = bool(self.ctx.nvls)
+        nvls = self._nvls_for(wire)
         if self.fused:
             kind = cu.OPT_SGD if self.fused == "sgd" else cu.OPT_ADAM
             hp_ptr = self._hp_dev.data_ptr() + 64 * b.group_index
@@ -516,6 +594,8 @@ class BucketedGradSync:
             mode = "batch" if (self.world > 1 and eligible) else "off"
         if mode != "off" and not eligible:
             mode = "off"
+        if mode == "persistent" and self.loss_scaler is not None:
+            mode = "batch"      # every exchange waits for the overflow decision at the step: nothing to start early
         self._ring_mode = mode
         if mode == "off":
             return
@@ -572,10 +652,10 @@ class BucketedGradSync:
         ev = torch.cuda.Event()
         ev.record(cur)
         cs.wait_event(ev)
-        nvls = bool(self.ctx.nvls) and self._reduce_engine != "lsu"
         i = 0
         while i < len(pend):
             b0 = pend[i]
+            nvls = self._nvls_for(self._wire(b0)) and self._reduce_engine != "lsu"
             j = i + 1
             while (j < len(pend) and pend[j].ring_cls == b0.ring_cls
                    and pend[j].ring_pos == pend[j - 1].ring_pos + 1):
@@ -688,12 +768,7 @@ class BucketedGradSync:
         if self._stamps:
             self.ctx.cu.ring_stamp(self.ctx.view, 0, cur.cuda_stream)       # backward (and everything before) done
             self._count_launch()
-        for b in self.buckets:
-            if not b.launched:      # unused parameters: issue in index order on every rank
-                self._zero_unused(b)
-                b.pending = 0
-                self._issue(b)
-        self._ring_flush()
+        self._issue_remaining()
         if self._stamps and self._last_done is not None:
             self.ctx.cu.ring_stamp(self.ctx.view, 1, self.comm_stream.cuda_stream)   # last exchange finished
             self._count_launch()
@@ -713,14 +788,58 @@ class BucketedGradSync:
             if self._delay.get(p) == self.bpps:
                 self._grad_views[p].zero_()
 
-    def finish_launches(self):
-        """Launch every bucket that has not gone out yet, without waiting."""
+    def _issue_remaining(self):
+        """Issue every bucket that has not gone out yet (unused parameters), in index order on every rank."""
+        if self.loss_scaler is not None:
+            self._issue_scaled_step()
+            return
         for b in self.buckets:
             if not b.launched:
                 self._zero_unused(b)
                 b.pending = 0
                 self._issue(b)
         self._ring_flush()
+
+    def _issue_scaled_step(self):
+        """Dynamic loss scaling: the whole exchange of the step, issued at the step on the comm stream.
+
+        1. loss_scale_check: does any element of this rank's gradient windows overflow on its wire?
+        2. loss_scale_update: every rank learns every rank's flag (barrier_peers, OR in rank order), updates the
+           scale, counts the step per group if it is applied, and writes grad_scale = 1/S, skip, first_step and the
+           Adam bias corrections into the hyper-parameter blocks, over what refresh_hparams put there.
+        3. every bucket's fused exchange in bucket order: one ring flush (BYTEPS_RING=batch, and persistent, which
+           behaves as batch here) or one launch per bucket; a skipped step leaves the optimizer state as it is.
+        The hooks launched nothing during backward, so the update no longer overlaps with it."""
+        for b in self.buckets:
+            if not b.launched:
+                self._zero_unused(b)
+                b.pending = 0
+        cu = self.ctx.cu
+        cur = torch.cuda.current_stream(self.device)
+        cs = self.comm_stream
+        ev = torch.cuda.Event()
+        ev.record(cur)
+        cs.wait_event(ev)
+        state = self._ls_state.data_ptr()
+        cu.loss_scale_check(self.ctx.view, self._ls_table.data_ptr(), len(self.buckets), self._ls_max_vectors, state,
+                            cs.cuda_stream)
+        cu.loss_scale_update(self.ctx.view, 0, self.ls_win_off, state, self._ls_steps.data_ptr(),
+                             self._ls_betas.data_ptr(), self._hp_dev.data_ptr(), len(self.param_groups),
+                             self.fused != "sgd", cs.cuda_stream)
+        self._count_launch(2)
+        for b in self.buckets:
+            if self._ring_mode != "off" and b.ring_cls is not None:
+                self._ring_pending.append(b)
+                b.launched = True
+                self._launched += 1
+            else:
+                self._ring_flush()          # keep the comm stream in bucket order
+                self._launch(b)
+        self._ring_flush()
+
+    def finish_launches(self):
+        """Launch every bucket that has not gone out yet, without waiting."""
+        self._issue_remaining()
         if self._stamps and self._last_done is not None:
             self.ctx.cu.ring_stamp(self.ctx.view, 1, self.comm_stream.cuda_stream)   # last exchange finished
             self._count_launch()
@@ -878,6 +997,8 @@ class BucketedGradSync:
                 copy_bucket_state(stage, (s0, s1), b.starts, tensors, to_shard=True)
                 buf.copy_(stage)
         self._group_step = [int(t) for t in group_steps]
+        if self.loss_scaler is not None:
+            self._ls_steps.copy_(torch.tensor(self._group_step, dtype=torch.int32))
         self.refresh_hparams()
 
     def close(self):

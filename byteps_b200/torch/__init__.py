@@ -17,6 +17,7 @@ parameters instead of the gradients.
 from __future__ import annotations
 
 import io
+import math
 import os
 from contextlib import contextmanager
 
@@ -61,10 +62,67 @@ def _fused_kind(optimizer_cls, param_groups):
     return None
 
 
+# torch.amp.GradScaler's defaults, by its names
+_LOSS_SCALE_DEFAULTS = {"init_scale": 65536.0, "growth_factor": 2.0, "backoff_factor": 0.5, "growth_interval": 2000}
+
+
+def _loss_scale_config(option):
+    """The dynamic_loss_scale argument as a complete dict of GradScaler's parameters, or None when it is off."""
+    if option is None or option is False:
+        return None
+    if option is True:
+        return dict(_LOSS_SCALE_DEFAULTS)
+    if not isinstance(option, dict):
+        raise ValueError("dynamic_loss_scale must be a bool or a dict of %s" % ", ".join(_LOSS_SCALE_DEFAULTS))
+    unknown = sorted(set(option) - set(_LOSS_SCALE_DEFAULTS))
+    if unknown:
+        raise ValueError("dynamic_loss_scale: unknown key(s) %s; expected some of %s"
+                         % (", ".join(map(repr, unknown)), ", ".join(_LOSS_SCALE_DEFAULTS)))
+    cfg = dict(_LOSS_SCALE_DEFAULTS, **option)
+    return dict(zip(_LOSS_SCALE_DEFAULTS, _checked_scaler_values(
+        "dynamic_loss_scale", cfg["init_scale"], cfg["growth_factor"], cfg["backoff_factor"], cfg["growth_interval"])))
+
+
+def _checked_scaler_entry(ls):
+    """A loaded "loss_scaler" entry (GradScaler.state_dict()'s keys) as (scale, growth_factor, backoff_factor,
+    growth_interval, growth_tracker), checked like the constructor's options, or ValueError."""
+    missing = sorted({"scale", "growth_factor", "backoff_factor", "growth_interval", "_growth_tracker"} - set(ls))
+    if missing:
+        raise ValueError("loaded loss_scaler entry lacks %s" % ", ".join(missing))
+    vals = _checked_scaler_values("loaded loss_scaler", ls["scale"], ls["growth_factor"], ls["backoff_factor"],
+                                  ls["growth_interval"])
+    tracker = ls["_growth_tracker"]
+    if isinstance(tracker, bool) or int(tracker) != tracker or not 0 <= tracker < vals[3]:
+        raise ValueError("loaded loss_scaler: _growth_tracker must be an integer in [0, growth_interval), got %r"
+                         % (tracker,))
+    return vals + (int(tracker),)
+
+
+def _checked_scaler_values(what, scale, growth, backoff, interval):
+    """(scale, growth_factor, backoff_factor, growth_interval) as float, float, float, int, or ValueError."""
+    scale, growth, backoff = float(scale), float(growth), float(backoff)
+    # the device holds S as a float32 and multiplies the gradients by the float32 1/S
+    s32 = float(torch.tensor(scale, dtype=torch.float32))
+    if not (math.isfinite(s32) and s32 > 0 and math.isfinite(float(torch.tensor(1.0 / s32, dtype=torch.float32)))):
+        raise ValueError("%s: the scale must be positive with S and 1/S finite in float32, got %r" % (what, scale))
+    if not growth > 1 or not math.isfinite(growth):
+        raise ValueError("%s: growth_factor must be finite and > 1, got %r" % (what, growth))
+    if not 0 < backoff < 1:
+        raise ValueError("%s: backoff_factor must be in (0, 1), got %r" % (what, backoff))
+    if isinstance(interval, bool) or int(interval) != interval or interval < 1:
+        raise ValueError("%s: growth_interval must be an integer >= 1, got %r" % (what, interval))
+    return scale, growth, backoff, int(interval)
+
+
 class _DistributedOptimizer(torch.optim.Optimizer):
     def __init__(self, params, named_parameters, compression, backward_passes_per_step=1, fused_update=None,
-                 bucket_bytes=None, compression_params=None):
+                 bucket_bytes=None, compression_params=None, dynamic_loss_scale=None):
         super(self.__class__, self).__init__(params)
+        if fused_update is None:
+            fused_update = os.getenv("BYTEPS_FUSED_OPTIMIZER", "0") not in ("0", "")
+        loss_scaler = _loss_scale_config(dynamic_loss_scale)
+        if loss_scaler is not None and not fused_update:
+            raise ValueError("dynamic_loss_scale needs fused_update=True")
         self._compression = compression
         from ..common.compression_params import translate
 
@@ -110,12 +168,14 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             set_learning_rate(self.param_groups[0]["lr"])
 
         eng = _engine()
-        if fused_update is None:
-            fused_update = os.getenv("BYTEPS_FUSED_OPTIMIZER", "0") not in ("0", "")
         on_cuda = all(p.is_cuda for p in all_params) and torch.cuda.is_available()
         # lossy compressors work per tensor (own error-feedback state): they take the per-parameter path
         want_symm = on_cuda and not self._enable_async and not self._compress_kwargs and (
             eng.backend == "symm" or (eng.backend == "local" and fused_update))
+        if loss_scaler is not None and not want_symm:
+            raise ValueError("dynamic_loss_scale needs the fused update on the symmetric-memory or local backend "
+                             "(CUDA parameters, no lossy compression, no BYTEPS_ENABLE_ASYNC); this job uses the %r "
+                             "backend" % eng.backend)
         if want_symm:
             from ..parallel.bucket import BucketedGradSync
 
@@ -126,7 +186,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             self._sync = BucketedGradSync(eng, self.param_groups, fused=kind, wire_dtype=_wire_of(compression),
                                           bucket_bytes=bucket_bytes,
                                           backward_passes_per_step=backward_passes_per_step,
-                                          priority_of=self._priority)
+                                          priority_of=self._priority, loss_scaler=loss_scaler)
             if kind:
                 self._sync.refresh_hparams()
         elif size() > 1 or eng.backend == "ps":
@@ -275,6 +335,30 @@ class _DistributedOptimizer(torch.optim.Optimizer):
     def grad_sync(self):
         return self._sync
 
+    # ---- dynamic loss scaling (fused mode) ------------------------------------------
+    def _scaler(self):
+        if self._sync is None or self._sync.loss_scaler is None:
+            raise RuntimeError("this optimizer was built without dynamic_loss_scale")
+        return self._sync
+
+    def scale_loss(self, loss):
+        """``loss * S``, S being the current loss scale as a device scalar: no host synchronisation, so it can be
+        captured into a CUDA graph.  Use ``opt.scale_loss(loss).backward()``; ``step()`` unscales, skips a step
+        whose gradients overflowed and updates S."""
+        return loss * self._scaler().scale_tensor()
+
+    @property
+    def loss_scale(self):
+        """The current loss scale S (a float).  Reads it from the device: synchronises."""
+        return self._scaler().loss_scaler_state()["scale"]
+
+    @property
+    def skipped_steps(self):
+        """Steps this optimizer skipped because a gradient overflowed.  Reads the count from the device:
+        synchronises.  The count is not part of a checkpoint: after ``load_state_dict`` it continues from this
+        optimizer's own count, not from the saved run's."""
+        return self._scaler().loss_scaler_state()["skipped"]
+
     def _drop_loaded_state(self):
         """Fused mode: forget the full copies of a load that no broadcast_optimizer_state consumed.  Training has
         moved on from them (a later broadcast must offer the live state, not roll back to the checkpoint)."""
@@ -300,10 +384,11 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         if not self._fused:
             return sd
         full = self._sync.export_state()
+        steps = self._sync.applied_steps()
         state = {}
         idx = 0
         for gi, g in enumerate(self.param_groups):
-            t = self._sync._group_step[gi]
+            t = steps[gi]
             for p in g["params"]:
                 ent = full.get(p)
                 if ent is not None:
@@ -322,7 +407,15 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                         state[idx] = e
                 idx += 1
         sd["state"] = state
+        if self._sync.loss_scaler is not None:
+            sd["loss_scaler"] = self._loss_scaler_entry()
         return sd
+
+    def _loss_scaler_entry(self):
+        """torch.amp.GradScaler.state_dict() of the device scaler."""
+        st = self._sync.loss_scaler_state()
+        return {"scale": st["scale"], "growth_factor": st["growth_factor"], "backoff_factor": st["backoff_factor"],
+                "growth_interval": st["growth_interval"], "_growth_tracker": st["tracker"]}
 
     def load_state_dict(self, state_dict):
         """Load a state dict of ``state_dict()`` or of the matching ``torch.optim`` optimizer.
@@ -337,6 +430,9 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         """
         if not self._fused:
             return super(self.__class__, self).load_state_dict(state_dict)
+        ls_vals = None
+        if self._sync.loss_scaler is not None and state_dict.get("loss_scaler") is not None:
+            ls_vals = _checked_scaler_entry(state_dict["loss_scaler"])    # before anything is installed
         live = [p for g in self.param_groups for p in g["params"]]
         saved = [i for g in state_dict["param_groups"] for i in g["params"]]
         by_id = dict(zip(saved, live))
@@ -365,6 +461,11 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             old.update(new)
         self.param_groups = groups
         self.state.update(full)
+        if self._sync.loss_scaler is not None:
+            if ls_vals is None:
+                self._sync.reset_loss_scaler()
+            else:
+                self._sync.set_loss_scaler_state(*ls_vals)
         keys = self._FUSED_KEYS[self._fused]
         self._sync.import_state({p: dict({"master": e.get("master_param")},
                                          **{"state%d" % i: e.get(k) for i, k in enumerate(keys)})
@@ -372,7 +473,8 @@ class _DistributedOptimizer(torch.optim.Optimizer):
 
 
 def DistributedOptimizer(optimizer, named_parameters=None, compression=Compression.none,
-                         backward_passes_per_step=1, fused_update=None, bucket_bytes=None, compression_params=None):
+                         backward_passes_per_step=1, fused_update=None, bucket_bytes=None, compression_params=None,
+                         dynamic_loss_scale=False):
     """Wrap ``optimizer`` so gradients are averaged over all processes before
     ``step()``; communication overlaps with ``loss.backward()``.
 
@@ -386,10 +488,20 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
 
     ``synchronize()`` forces completion (e.g. before gradient clipping),
     ``skip_synchronize()`` lets a following ``step()`` skip it.
+
+    ``dynamic_loss_scale`` (with ``fused_update=True``, symmetric-memory or local backend): dynamic loss scaling
+    for fp16 training, decided on the device.  ``True`` uses ``torch.amp.GradScaler``'s defaults; a dict overrides
+    any of ``init_scale``, ``growth_factor``, ``backoff_factor`` and ``growth_interval`` (GradScaler's meanings).
+    The loop is ``opt.zero_grad(); opt.scale_loss(loss).backward(); opt.step()``: a step whose gradients hold an
+    inf or NaN on any rank (as they go onto the wire) is skipped on every rank and the scale backs off; the scale
+    grows after ``growth_interval`` clean steps.  Nothing synchronises with the host, so the step captures into a
+    CUDA graph.  ``loss_scale`` and ``skipped_steps`` read the state (and synchronise); ``state_dict()`` carries
+    it as ``"loss_scaler"`` in GradScaler's format.  Do not combine ``fused_update=True`` with a
+    ``torch.amp.GradScaler``: the update happens inside the exchange, before the scaler could unscale or skip it.
     """
     cls = type(optimizer.__class__.__name__, (optimizer.__class__,), dict(_DistributedOptimizer.__dict__))
     return cls(optimizer.param_groups, named_parameters, compression, backward_passes_per_step, fused_update,
-               bucket_bytes, compression_params)
+               bucket_bytes, compression_params, dynamic_loss_scale)
 
 
 def broadcast_parameters(params, root_rank, prefix="Parameter."):
@@ -509,7 +621,12 @@ def broadcast_optimizer_state(optimizer, root_rank, prefix="Parameter."):
                 else:
                     plain["state"].setdefault(pid, {})[field] = val
     broadcast_parameters(tensors, root_rank, prefix)
+    if fused and optimizer.grad_sync.loss_scaler is not None:
+        # the root's scaler: what its load_state_dict installed, or its live state
+        plain["loss_scaler"] = optimizer._loss_scaler_entry() if rank() == root_rank else None
     plain = broadcast_object(plain, root_rank, name="optimizer_state.plain")
+    if "loss_scaler" in plain:
+        sd["loss_scaler"] = plain["loss_scaler"]
     for live, stored, opts in zip(optimizer.param_groups, sd["param_groups"], plain["groups"]):
         live.update(opts)
         stored.update(opts)             # load_state_dict below must not put the old options back
