@@ -12,11 +12,17 @@ are the least each fused pass must move, computed from the shape (e = element by
     bwd_reduce  read dy, x [, mask]                       2 N e [+ N / 8]
     bwd_apply   read dy, x [, mask]; write dx [, dres]    N e (3 [+1]) [+ N / 8]
 
-The stock rows time F.batch_norm [+ add] [+ relu] and its autograd backward; their GB/s use the fused passes'
+    single:fwd  read x once [, residual]; write y [, mask]  N e (2 [+1]) [+ N / 8]   (fwd_stats + fwd_apply in one launch)
+    single:bwd  read dy, x [, mask] once; write dx [, dres]  N e (3 [+1]) [+ N / 8]   (bwd_reduce + bwd_apply)
+
+The fused:fwd / fused:bwd rows sum the two-pass kernels; the single rows are the single-launch kernels the module
+takes where their plan allows it.  Every timed launch moves to the next of enough copies of the tensors that the
+launches of a row touch more than --rotate-mb together, so no pass finds its input in the 50 MB L2 from the launch
+before.  The stock rows time F.batch_norm [+ add] [+ relu] and its autograd backward; their GB/s use the fused passes'
 bytes, i.e. they are the rate at which the stock sequence delivers the same work.  Share of peak is against the
 H100 SXM data-sheet 3.35 TB/s; the GPU name and power limit are printed with the table.
 
-    python benchmarks/bn_act_bench.py [--batch 64] [--iters 50] [--json out.json]
+    python benchmarks/bn_act_bench.py [--batch 64] [--iters 50] [--rotate-mb 200] [--json out.json]
 """
 import argparse
 import json
@@ -48,6 +54,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=64)
     ap.add_argument("--iters", type=int, default=50)
+    ap.add_argument("--rotate-mb", type=float, default=200.0, help="bytes the tensor copies of a row span together")
     ap.add_argument("--json", default=None, help="also write the rows as JSON to this file")
     args = ap.parse_args()
 
@@ -64,13 +71,14 @@ def main():
     s = torch.cuda.current_stream().cuda_stream
     dt, code, e = torch.bfloat16, 1, 2
 
-    def timed(fn):
-        for _ in range(3):
-            fn()
+    def timed(fn, k):
+        """fn(i) on tensor copy i % k"""
+        for i in range(max(3, k)):
+            fn(i % k)
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
-        for _ in range(args.iters):
-            fn()
+        for i in range(args.iters):
+            fn(i % k)
         b.record()
         torch.cuda.synchronize()
         return a.elapsed_time(b) / args.iters
@@ -85,63 +93,98 @@ def main():
         for var in variants:
             relu, res = var != "none", var == "relu_res"
             g = torch.Generator(device=dev).manual_seed(0)
-            x = torch.randn(args.batch, c, h, w, device=dev, generator=g).to(dt).contiguous(
-                memory_format=torch.channels_last)
-            r = torch.randn_like(x) if res else None
-            dy = torch.randn_like(x)
+            mb = n // 8 if relu else 0
+            k = max(1, int(-(-args.rotate_mb * 1e6 // (n * e * (5 if res else 3) + 2 * mb))))
+
+            def copies():
+                x = torch.randn(args.batch, c, h, w, device=dev, generator=g).to(dt).contiguous(
+                    memory_format=torch.channels_last)
+                return dict(x=x, r=torch.randn_like(x) if res else None, dy=torch.randn_like(x),
+                            y=torch.empty_like(x), dx=torch.empty_like(x),
+                            dres=torch.empty_like(x) if res else None,
+                            mask=torch.empty(m, c // 8, dtype=torch.uint8, device=dev) if relu else None)
+
+            T = [copies() for _ in range(k)]
+            P = [{key: (0 if t is None else t.data_ptr()) for key, t in tk.items()} for tk in T]
             wt, bs = torch.ones(c, device=dev), torch.zeros(c, device=dev)
             rm, rv = torch.zeros(c, device=dev), torch.ones(c, device=dev)
             mean, inv, dw, db = (torch.empty(c, device=dev) for _ in range(4))
             nws, nctr = cu.bn_act_workspace(m, c)
             ws = torch.empty(nws, device=dev)
             ctr = torch.zeros(nctr, dtype=torch.int32, device=dev)
-            y, dx = torch.empty_like(x), torch.empty_like(x)
-            dres = torch.empty_like(x) if res else None
-            mask = torch.empty(m, c // 8, dtype=torch.uint8, device=dev) if relu else None
-            mp, rp, dp = (mask.data_ptr() if relu else 0), (r.data_ptr() if res else 0), (dres.data_ptr() if res else 0)
-            mb = n // 8 if relu else 0
             passes = [
-                ("fwd_stats", n * e, lambda: cu.bn_act_fwd_stats(x.data_ptr(), code, m, c, 1e-5, 0.1, rm.data_ptr(),
-                                                                 rv.data_ptr(), mean.data_ptr(), inv.data_ptr(),
-                                                                 ws.data_ptr(), ctr.data_ptr(), s)),
+                ("fwd_stats", n * e, lambda i: cu.bn_act_fwd_stats(P[i]["x"], code, m, c, 1e-5, 0.1, rm.data_ptr(),
+                                                                   rv.data_ptr(), mean.data_ptr(), inv.data_ptr(),
+                                                                   ws.data_ptr(), ctr.data_ptr(), s)),
                 ("fwd_apply", n * e * (3 if res else 2) + mb,
-                 lambda: cu.bn_act_fwd_apply(x.data_ptr(), rp, code, m, c, mean.data_ptr(), inv.data_ptr(),
-                                             wt.data_ptr(), bs.data_ptr(), relu, y.data_ptr(), mp, s)),
+                 lambda i: cu.bn_act_fwd_apply(P[i]["x"], P[i]["r"], code, m, c, mean.data_ptr(), inv.data_ptr(),
+                                               wt.data_ptr(), bs.data_ptr(), relu, P[i]["y"], P[i]["mask"], s)),
                 ("bwd_reduce", 2 * n * e + mb,
-                 lambda: cu.bn_act_bwd_reduce(dy.data_ptr(), x.data_ptr(), mp, code, m, c, mean.data_ptr(),
-                                              inv.data_ptr(), dw.data_ptr(), db.data_ptr(), ws.data_ptr(),
-                                              ctr.data_ptr(), s)),
+                 lambda i: cu.bn_act_bwd_reduce(P[i]["dy"], P[i]["x"], P[i]["mask"], code, m, c, mean.data_ptr(),
+                                                inv.data_ptr(), dw.data_ptr(), db.data_ptr(), ws.data_ptr(),
+                                                ctr.data_ptr(), s)),
                 ("bwd_apply", n * e * (4 if res else 3) + mb,
-                 lambda: cu.bn_act_bwd_apply(dy.data_ptr(), x.data_ptr(), mp, code, m, c, mean.data_ptr(),
-                                             inv.data_ptr(), wt.data_ptr(), dw.data_ptr(), db.data_ptr(),
-                                             dx.data_ptr(), dp, s)),
+                 lambda i: cu.bn_act_bwd_apply(P[i]["dy"], P[i]["x"], P[i]["mask"], code, m, c, mean.data_ptr(),
+                                               inv.data_ptr(), wt.data_ptr(), dw.data_ptr(), db.data_ptr(),
+                                               P[i]["dx"], P[i]["dres"], s)),
             ]
             tot = {"fwd": [0.0, 0], "bwd": [0.0, 0]}
             for name, nbytes, fn in passes:
-                ms = timed(fn)
+                ms = timed(fn, k)
                 side = tot[name[:3]]
                 side[0] += ms
                 side[1] += nbytes
                 rows.append(dict(shape=[c, h, w], variant=var, impl="fused", kind=name, bytes=nbytes, us=ms * 1e3))
 
+            # the single-launch kernels; their counters are left non-zero, so each launch gets a zeroed set
+            fplan, bplan = cu.bn_act_plan(0, code, m, c), cu.bn_act_plan(1, code, m, c)
+            single = []
+            if fplan is not None and bplan is not None:
+                nctr1 = max(fplan["counters"], bplan["counters"])
+                ws1 = torch.empty(max(fplan["ws_floats"], bplan["ws_floats"]), device=dev)
+                ctrs = torch.zeros(args.iters + max(3, k), nctr1, dtype=torch.int32, device=dev)
+                launch = [0]
+
+                def zeroed():
+                    launch[0] += 1
+                    return ctrs[launch[0] - 1].data_ptr()
+
+                single = [
+                    ("fwd", n * e * (3 if res else 2) + mb,
+                     lambda i: cu.bn_act_fwd(P[i]["x"], P[i]["r"], code, m, c, 1e-5, 0.1, rm.data_ptr(), rv.data_ptr(),
+                                             mean.data_ptr(), inv.data_ptr(), wt.data_ptr(), bs.data_ptr(), relu,
+                                             P[i]["y"], P[i]["mask"], ws1.data_ptr(), zeroed(), s)),
+                    ("bwd", n * e * (4 if res else 3) + mb,
+                     lambda i: cu.bn_act_bwd(P[i]["dy"], P[i]["x"], P[i]["mask"], code, m, c, mean.data_ptr(),
+                                             inv.data_ptr(), wt.data_ptr(), dw.data_ptr(), db.data_ptr(), P[i]["dx"],
+                                             P[i]["dres"], ws1.data_ptr(), zeroed(), s)),
+                ]
+                for name, nbytes, fn in single:
+                    launch[0] = 0
+                    ctrs.zero_()
+                    ms = timed(fn, k)
+                    rows.append(dict(shape=[c, h, w], variant=var, impl="single", kind=name, bytes=nbytes,
+                                     us=ms * 1e3, held_rows=(fplan if name == "fwd" else bplan)["held_rows"],
+                                     rows_per_chunk=fplan["rows_per_chunk"]))
+
             # stock sequence on the same tensors
-            xs = x.detach().requires_grad_(True)
-            rs = r.detach().requires_grad_(True) if res else None
+            XS = [t["x"].detach().requires_grad_(True) for t in T]
+            RS = [t["r"].detach().requires_grad_(True) if res else None for t in T]
             ws_, bs_ = wt.clone().requires_grad_(True), bs.clone().requires_grad_(True)
 
-            def stock_fwd():
-                t = F.batch_norm(xs, rm, rv, ws_, bs_, True, 0.1, 1e-5)
+            def stock_fwd(i):
+                t = F.batch_norm(XS[i], rm, rv, ws_, bs_, True, 0.1, 1e-5)
                 if res:
-                    t = t + rs
+                    t = t + RS[i]
                 return F.relu(t, inplace=True) if relu else t
 
-            def stock_both():
-                t = stock_fwd()
-                torch.autograd.grad(t, [xs, ws_, bs_] + ([rs] if res else []), dy)
+            def stock_both(i):
+                t = stock_fwd(i)
+                torch.autograd.grad(t, [XS[i], ws_, bs_] + ([RS[i]] if res else []), T[i]["dy"])
 
             with torch.no_grad():
-                ms_f = timed(stock_fwd)
-            ms_b = timed(stock_both) - timed(stock_fwd)
+                ms_f = timed(stock_fwd, k)
+            ms_b = timed(stock_both, k) - timed(stock_fwd, k)
             rows.append(dict(shape=[c, h, w], variant=var, impl="stock", kind="fwd", bytes=tot["fwd"][1],
                              us=ms_f * 1e3))
             rows.append(dict(shape=[c, h, w], variant=var, impl="stock", kind="bwd", bytes=tot["bwd"][1],
@@ -149,15 +192,17 @@ def main():
             for side in ("fwd", "bwd"):
                 rows.append(dict(shape=[c, h, w], variant=var, impl="fused", kind=side, bytes=tot[side][1],
                                  us=tot[side][0] * 1e3))
-            for row in rows[-(len(passes) + 4):]:
+            for row in rows[-(len(passes) + len(single) + 4):]:
                 gbs = row["bytes"] / (row["us"] * 1e3)
                 row["gbs"], row["peak_share"] = gbs, gbs / PEAK_GBS
                 print("%-14s %-9s %-11s %9.1f %9.1f %8.0f %5.0f%%" % (
                     "%dx%dx%d" % (c, h, w), var, row["impl"] + ":" + row["kind"], row["bytes"] / 1e6, row["us"], gbs,
                     100 * row["peak_share"]))
+            del T, P, XS, RS
     f_tot = sum(r_["us"] for r_ in rows if r_["impl"] == "fused" and r_["kind"] in ("fwd", "bwd"))
+    g_tot = sum(r_["us"] for r_ in rows if r_["impl"] == "single")
     s_tot = sum(r_["us"] for r_ in rows if r_["impl"] == "stock")
-    print("sum over the variants above: fused %.0f us, stock %.0f us" % (f_tot, s_tot))
+    print("sum over the variants above: two-pass %.0f us, single-launch %.0f us, stock %.0f us" % (f_tot, g_tot, s_tot))
     if args.json:
         with open(args.json, "w") as fh:
             json.dump({"gpu": info, "batch": args.batch, "rows": rows}, fh, indent=1)

@@ -59,6 +59,45 @@ void bind_cuda_bn(py::module_& m) {
      py::arg("stream"), py::arg("total") = 0,
      "total: device float holding the row count to divide by (bn_sync_stats writes it); 0 divides by M");
 
+  // ---- single-launch passes
+  m.def("bn_act_plan", [](int bwd, int dtype, size_t M, int C, long long cap) -> py::object {
+    BnFusedPlan p;
+    if (!bn_act_fused_plan(bwd, dtype, M, C, cap, &p)) return py::none();
+    py::dict d;
+    d["ws_floats"] = p.ws_floats;
+    d["counters"] = p.counters;
+    d["rows_per_chunk"] = p.rows_per_chunk;
+    d["held_rows"] = p.held_rows;
+    d["held_bytes"] = p.held_bytes;
+    d["wave_blocks"] = p.wave_blocks;
+    return d;
+  }, py::arg("bwd"), py::arg("dtype"), py::arg("M"), py::arg("C"), py::arg("cap") = -1,
+     "plan of the single-launch bn_act_fwd (bwd=0) / bn_act_bwd (bwd=1) at (M, C, dtype) on the current device, or "
+     "None when it cannot run there; cap >= 0 limits the bytes of rows a block holds in shared memory");
+  m.def("bn_act_fwd", [](uintptr_t x, uintptr_t residual, int dtype, size_t M, int C, float eps, float momentum,
+                         uintptr_t running_mean, uintptr_t running_var, uintptr_t save_mean, uintptr_t save_invstd,
+                         uintptr_t weight, uintptr_t bias, bool relu, uintptr_t y, uintptr_t mask, uintptr_t ws,
+                         uintptr_t counters, uintptr_t s, long long cap) {
+    chk(launch_bn_act_fwd((const void*)x, (const void*)residual, dtype, M, C, eps, momentum, (float*)running_mean,
+                          (float*)running_var, (float*)save_mean, (float*)save_invstd, (const float*)weight,
+                          (const float*)bias, relu ? 1 : 0, (void*)y, (uint8_t*)mask, (float*)ws, (uint32_t*)counters,
+                          cap, (cudaStream_t)s),
+        "bn_act_fwd");
+  }, py::arg("x"), py::arg("residual"), py::arg("dtype"), py::arg("M"), py::arg("C"), py::arg("eps"),
+     py::arg("momentum"), py::arg("running_mean"), py::arg("running_var"), py::arg("save_mean"),
+     py::arg("save_invstd"), py::arg("weight"), py::arg("bias"), py::arg("relu"), py::arg("y"), py::arg("mask"),
+     py::arg("ws"), py::arg("counters"), py::arg("stream"), py::arg("cap") = -1);
+  m.def("bn_act_bwd", [](uintptr_t dy, uintptr_t x, uintptr_t mask, int dtype, size_t M, int C, uintptr_t mean,
+                         uintptr_t invstd, uintptr_t weight, uintptr_t dweight, uintptr_t dbias, uintptr_t dx,
+                         uintptr_t dresidual, uintptr_t ws, uintptr_t counters, uintptr_t s, long long cap) {
+    chk(launch_bn_act_bwd((const void*)dy, (const void*)x, (const uint8_t*)mask, dtype, M, C, (const float*)mean,
+                          (const float*)invstd, (const float*)weight, (float*)dweight, (float*)dbias, (void*)dx,
+                          (void*)dresidual, (float*)ws, (uint32_t*)counters, cap, (cudaStream_t)s),
+        "bn_act_bwd");
+  }, py::arg("dy"), py::arg("x"), py::arg("mask"), py::arg("dtype"), py::arg("M"), py::arg("C"), py::arg("mean"),
+     py::arg("invstd"), py::arg("weight"), py::arg("dweight"), py::arg("dbias"), py::arg("dx"), py::arg("dresidual"),
+     py::arg("ws"), py::arg("counters"), py::arg("stream"), py::arg("cap") = -1);
+
   // ---- synchronised batch norm
   m.def("bn_act_load_kernels", []() { chk(bn_act_load_kernels(), "bn_act_load_kernels"); },
         "load every batch-norm kernel variant now (before any cross-rank launch)");

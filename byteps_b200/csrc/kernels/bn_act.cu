@@ -7,6 +7,8 @@
 // live in registers, and a warp touches 512 contiguous bytes of a 16-bit row when C >= 256.
 #include "kernels/bn_act.cuh"
 
+#include <mutex>
+
 #include "kernels/common.cuh"
 #include "kernels/pushpull.cuh"
 
@@ -182,6 +184,33 @@ struct Fin {
   }
 };
 
+// Merge of the G chunk partials (chunk g: rpc rows, the last M - (G - 1) rpc) of channel c with Chan's formula for
+// G parts: mean = sum n_g mean_g / M, M2 = sum (M2_g + n_g (mean_g - mean)^2), two fixed-order sums.  ws holds the
+// chunk means, then the chunk M2s, G x C each.  Every thread of the block must call it; lanes of c >= C get 0.
+__device__ __forceinline__ void merge_stats(const Fin& fin, const float* ws, int G, size_t M, int C, int c,
+                                            size_t rpc, float* fmean, float* fm2) {
+  const float* ws_mean = ws;
+  const float* ws_m2 = ws + (size_t)G * C;
+  const bool live = c < C;
+  const float rpcf = (float)rpc, last_n = (float)(M - (size_t)(G - 1) * rpc);
+  float a = 0.f;
+  if (live) {
+#pragma unroll 8
+    for (int g = fin.sub; g < G; g += fin.tpc) a += (g == G - 1 ? last_n : rpcf) * __ldcg(ws_mean + (size_t)g * C + c);
+  }
+  const float mean = fin.all_sum(a) / (float)M;
+  a = 0.f;
+  if (live) {
+#pragma unroll 8
+    for (int g = fin.sub; g < G; g += fin.tpc) {
+      const float d = __ldcg(ws_mean + (size_t)g * C + c) - mean;
+      a += __ldcg(ws_m2 + (size_t)g * C + c) + (g == G - 1 ? last_n : rpcf) * d * d;
+    }
+  }
+  *fmean = mean;
+  *fm2 = fin.all_sum(a);
+}
+
 // kLocal: local-partials mode of synchronised batch norm - save_mean / save_invstd receive this rank's mean and
 // M2 over its M rows (M >= 1), and the running statistics are left to bn_sync_kernel.
 template <class U, bool kLocal>
@@ -224,27 +253,12 @@ __global__ void __launch_bounds__(kT, kBlocksPerSM) bn_act_fwd_stats_kernel(cons
   }
   if (!last_block(counters + blockIdx.y)) return;
 
-  // The last chunk of this channel group to finish merges the group's G partials with Chan's formula for G parts:
-  // mean = sum n_g mean_g / M, M2 = sum (M2_g + n_g (mean_g - mean)^2), two fixed-order sums.
+  // The last chunk of this channel group to finish merges the group's G partials.
   const Fin fin(CB);
   const int c = blockIdx.y * fin.nc + fin.cl;
   const bool live = c < C;
-  const float rpcf = (float)rpc, last_n = (float)(M - (size_t)(G - 1) * rpc);
-  float a = 0.f;
-  if (live) {
-#pragma unroll 8
-    for (int g = fin.sub; g < G; g += fin.tpc) a += (g == G - 1 ? last_n : rpcf) * __ldcg(ws_mean + (size_t)g * C + c);
-  }
-  const float fmean = fin.all_sum(a) / (float)M;
-  a = 0.f;
-  if (live) {
-#pragma unroll 8
-    for (int g = fin.sub; g < G; g += fin.tpc) {
-      const float d = __ldcg(ws_mean + (size_t)g * C + c) - fmean;
-      a += __ldcg(ws_m2 + (size_t)g * C + c) + (g == G - 1 ? last_n : rpcf) * d * d;
-    }
-  }
-  const float fm2 = fin.all_sum(a);
+  float fmean, fm2;
+  merge_stats(fin, ws, G, M, C, c, rpc, &fmean, &fm2);
   if constexpr (kLocal) {
     if (fin.sub == 0 && live) {
       save_mean[c] = fmean;
@@ -455,6 +469,314 @@ __global__ void __launch_bounds__(kT, kBwdApplyBlocksPerSM) bn_act_bwd_apply_ker
   }
 }
 
+// ---- single-launch passes: reduction, grid barrier, merge and apply in one cooperative launch ----------------
+//
+// The grid is exactly one wave of kResBlocksPerSM blocks per SM, laid out as the reduction passes: channel group
+// blockIdx.y, chunk blockIdx.x of rpc rows, thread (col, lane) on rows lane, lane + RL, ... of the chunk.  The first
+// `held` rows of a chunk (a multiple of RL, or the whole chunk) are copied into shared memory in phase 1 and applied
+// from there in phase 2; the rest are read from global memory in both phases, the second time in reverse order so
+// that what phase 1 read last, the part most likely still in L2, is read first.  Between the phases every block of a
+// channel group waits for the group's partials and merges them itself, in the same fixed order, so all of the group's
+// blocks get the same bits without a second barrier.
+constexpr int kResBlocksPerSM = 2;
+constexpr int kMaxRedCh = 8 * kCh;   // channels of a reduction-layout channel group (red_cb <= 8 units)
+
+__device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
+  uint32_t v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void cp_async16(void* smem, const void* g) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem)), "l"(g) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+// One-shot barrier of the gridDim.x blocks of a channel group on a zeroed counter.  Only cooperative launches use
+// it, so every block is resident and the wait ends; the time limit turns a broken launch into an error, not a hang.
+__device__ __forceinline__ void group_barrier(uint32_t* counter) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    atomicAdd(counter, 1u);
+    const long long t0 = clock64();
+    while (ld_acquire_gpu(counter) < gridDim.x) {
+      if (clock64() - t0 > kBarrierSpinLimit) {
+        printf("byteps_b200: bn_act block (%d, %d) timed out at its grid barrier\n", (int)blockIdx.x, (int)blockIdx.y);
+        __trap();
+      }
+    }
+  }
+  __syncthreads();
+}
+
+template <class U>
+__device__ __forceinline__ void hold_load(const Vec16* h, float* f) {
+#pragma unroll
+  for (int v = 0; v < Unit<U>::kVecs; ++v) U::unpack(lds16(h + v), f + v * U::kPerVec);
+}
+template <class U>
+__device__ __forceinline__ void hold_copy(Vec16* h, const void* base, size_t unit) {
+  const Vec16* p = reinterpret_cast<const Vec16*>(base) + unit * Unit<U>::kVecs;
+#pragma unroll
+  for (int v = 0; v < Unit<U>::kVecs; ++v) cp_async16(h + v, p + v);
+}
+
+// Dynamic shared memory: x of `held` block rows, CB units each.
+template <class U, bool kRelu, bool kRes>
+__global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_fwd_fused_kernel(
+    const void* __restrict__ x, const void* __restrict__ res, size_t M, int C, int shift, size_t rpc, int held,
+    float eps, float momentum, float* run_mean, float* run_var, float* save_mean, float* save_invstd,
+    const float* weight, const float* bias, void* y, uint8_t* mask, float* ws, uint32_t* counters) {
+  extern __shared__ Vec16 hold[];
+  constexpr int V = Unit<U>::kVecs;
+  __shared__ float s_mu[kMaxRedCh], s_sc[kMaxRedCh];
+  const int units = C / kCh, CB = 1 << shift, RL = kT >> shift;
+  const int col = threadIdx.x & (CB - 1), lane = threadIdx.x >> shift;
+  const int u = blockIdx.y * CB + col;
+  const size_t r0 = (size_t)blockIdx.x * rpc, r1 = min(M, r0 + rpc);
+  const int rows = (int)(r1 - r0), nh = min(held, rows);
+
+  // phase 1: held rows to shared memory, streamed rows through registers; Welford over all of them
+  float n = 0.f, mean[kCh], m2[kCh];
+#pragma unroll
+  for (int k = 0; k < kCh; ++k) mean[k] = m2[k] = 0.f;
+  if (u < units) {
+    for (int j = lane; j < nh; j += RL) hold_copy<U>(hold + (j * CB + col) * V, x, (r0 + j) * units + u);
+    size_t r = r0 + nh + lane;
+    for (; r + 3 * RL < r1; r += 4 * RL) {
+      float f[4][kCh];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) Unit<U>::load(x, (r + j * RL) * units + u, f[j]);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) welford_push(n, mean, m2, f[j]);
+    }
+    for (; r < r1; r += RL) {
+      float f[kCh];
+      Unit<U>::load(x, r * units + u, f);
+      welford_push(n, mean, m2, f);
+    }
+    cp_async_wait_all();
+    for (int j = lane; j < nh; j += RL) {
+      float f[kCh];
+      hold_load<U>(hold + (j * CB + col) * V, f);
+      welford_push(n, mean, m2, f);
+    }
+  }
+  tree_welford<kCh>(n, mean, m2, lane, CB, RL);
+  const int G = gridDim.x;
+  if (lane == 0 && u < units) {
+#pragma unroll
+    for (int k = 0; k < kCh; ++k) {
+      ws[(size_t)blockIdx.x * C + u * kCh + k] = mean[k];
+      ws[((size_t)G + blockIdx.x) * C + u * kCh + k] = m2[k];
+    }
+  }
+  group_barrier(counters + blockIdx.y);
+
+  const Fin fin(CB);
+  const int c = blockIdx.y * fin.nc + fin.cl;
+  float fmean, fm2;
+  merge_stats(fin, ws, G, M, C, c, rpc, &fmean, &fm2);
+  if (fin.sub == 0 && c < C) {
+    const float invstd = 1.f / sqrtf(fm2 / (float)M + eps);
+    s_mu[fin.cl] = fmean;
+    s_sc[fin.cl] = weight[c] * invstd;
+    if (blockIdx.x == 0) {
+      save_mean[c] = fmean;
+      save_invstd[c] = invstd;
+      if (run_mean != nullptr) {
+        run_mean[c] = momentum * fmean + (1.f - momentum) * run_mean[c];
+        run_var[c] = momentum * (fm2 / (float)(M - 1)) + (1.f - momentum) * run_var[c];
+      }
+    }
+  }
+  __syncthreads();
+  if (u >= units) return;
+
+  // phase 2: streamed rows, last read first, then the held rows
+  float mu[kCh], sc[kCh], sh[kCh];
+#pragma unroll
+  for (int k = 0; k < kCh; ++k) {
+    mu[k] = s_mu[col * kCh + k];
+    sc[k] = s_sc[col * kCh + k];
+    sh[k] = bias[u * kCh + k];
+  }
+  const int ns = rows - nh;
+  for (int k = lane < ns ? (ns - 1 - lane) / RL : -1; k >= 0; k -= 2) {
+    const size_t i0 = (r0 + nh + lane + (size_t)k * RL) * units + u, i1 = i0 - (size_t)RL * units;
+    float f0[kCh], f1[kCh], q0[kCh], q1[kCh];
+    Unit<U>::load(x, i0, f0);
+    if constexpr (kRes) Unit<U>::load(res, i0, q0);
+    if (k >= 1) {
+      Unit<U>::load(x, i1, f1);
+      if constexpr (kRes) Unit<U>::load(res, i1, q1);
+    }
+    fwd_row<U, kRelu, kRes>(i0, mu, sc, sh, y, mask, f0, q0);
+    if (k >= 1) fwd_row<U, kRelu, kRes>(i1, mu, sc, sh, y, mask, f1, q1);
+  }
+  for (int j = lane; j < nh; j += 2 * RL) {
+    const size_t i0 = (r0 + j) * units + u, i1 = i0 + (size_t)RL * units;
+    const bool two = j + RL < nh;
+    float f0[kCh], f1[kCh], q0[kCh], q1[kCh];
+    if constexpr (kRes) {
+      Unit<U>::load(res, i0, q0);
+      if (two) Unit<U>::load(res, i1, q1);
+    }
+    hold_load<U>(hold + (j * CB + col) * V, f0);
+    fwd_row<U, kRelu, kRes>(i0, mu, sc, sh, y, mask, f0, q0);
+    if (two) {
+      hold_load<U>(hold + ((j + RL) * CB + col) * V, f1);
+      fwd_row<U, kRelu, kRes>(i1, mu, sc, sh, y, mask, f1, q1);
+    }
+  }
+}
+
+// Dynamic shared memory: dy, then x of `held` block rows (CB units each), then their mask bytes.
+template <class U, bool kRelu, bool kRes>
+__global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_bwd_fused_kernel(
+    const void* __restrict__ dy, const void* __restrict__ x, const uint8_t* __restrict__ mask, size_t M, int C,
+    int shift, size_t rpc, int held, const float* mean, const float* invstd, const float* weight, float* dweight,
+    float* dbias, void* dx, void* dres, float* ws, uint32_t* counters) {
+  extern __shared__ Vec16 hold[];
+  constexpr int V = Unit<U>::kVecs;
+  __shared__ float s_A[kMaxRedCh], s_D[kMaxRedCh], s_E[kMaxRedCh];
+  const int units = C / kCh, CB = 1 << shift, RL = kT >> shift;
+  const int col = threadIdx.x & (CB - 1), lane = threadIdx.x >> shift;
+  const int u = blockIdx.y * CB + col;
+  const size_t r0 = (size_t)blockIdx.x * rpc, r1 = min(M, r0 + rpc);
+  const int rows = (int)(r1 - r0), nh = min(held, rows);
+  Vec16* hdy = hold;
+  Vec16* hx = hold + (size_t)held * CB * V;
+  uint8_t* hm = reinterpret_cast<uint8_t*>(hx + (size_t)held * CB * V);
+
+  // phase 1
+  float sg[kCh], sgx[kCh], mu[kCh];
+#pragma unroll
+  for (int k = 0; k < kCh; ++k) sg[k] = sgx[k] = 0.f;
+  if (u < units) {
+#pragma unroll
+    for (int k = 0; k < kCh; ++k) mu[k] = mean[u * kCh + k];
+    for (int j = lane; j < nh; j += RL) {
+      const size_t i = (r0 + j) * units + u;
+      hold_copy<U>(hdy + (j * CB + col) * V, dy, i);
+      hold_copy<U>(hx + (j * CB + col) * V, x, i);
+      if constexpr (kRelu) hm[j * CB + col] = mask[i];
+    }
+    size_t r = r0 + nh + lane;
+    for (; r + 3 * RL < r1; r += 4 * RL) {
+      float d[4][kCh], f[4][kCh];
+      uint32_t bits[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const size_t i = (r + j * RL) * units + u;
+        Unit<U>::load(dy, i, d[j]);
+        Unit<U>::load(x, i, f[j]);
+        if constexpr (kRelu) bits[j] = mask[i];
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        mask_grad<kRelu>(d[j], bits[j]);
+#pragma unroll
+        for (int k = 0; k < kCh; ++k) {
+          sg[k] += d[j][k];
+          sgx[k] = fmaf(d[j][k], f[j][k] - mu[k], sgx[k]);
+        }
+      }
+    }
+    for (; r < r1; r += RL) {
+      const size_t i = r * units + u;
+      float d[kCh], f[kCh];
+      Unit<U>::load(dy, i, d);
+      Unit<U>::load(x, i, f);
+      if constexpr (kRelu) mask_grad<kRelu>(d, mask[i]);
+#pragma unroll
+      for (int k = 0; k < kCh; ++k) {
+        sg[k] += d[k];
+        sgx[k] = fmaf(d[k], f[k] - mu[k], sgx[k]);
+      }
+    }
+    cp_async_wait_all();
+    for (int j = lane; j < nh; j += RL) {
+      float d[kCh], f[kCh];
+      hold_load<U>(hdy + (j * CB + col) * V, d);
+      hold_load<U>(hx + (j * CB + col) * V, f);
+      if constexpr (kRelu) mask_grad<kRelu>(d, hm[j * CB + col]);
+#pragma unroll
+      for (int k = 0; k < kCh; ++k) {
+        sg[k] += d[k];
+        sgx[k] = fmaf(d[k], f[k] - mu[k], sgx[k]);
+      }
+    }
+  }
+  tree_sum2<kCh>(sg, sgx, lane, CB, RL);
+  const int G = gridDim.x;
+  if (lane == 0 && u < units) {
+#pragma unroll
+    for (int k = 0; k < kCh; ++k) {
+      ws[(size_t)blockIdx.x * C + u * kCh + k] = sg[k];
+      ws[((size_t)G + blockIdx.x) * C + u * kCh + k] = sgx[k];
+    }
+  }
+  group_barrier(counters + blockIdx.y);
+
+  const Fin fin(CB);
+  const int c = blockIdx.y * fin.nc + fin.cl;
+  float a = 0.f, b = 0.f;
+  if (c < C) {
+#pragma unroll 8
+    for (int g = fin.sub; g < G; g += fin.tpc) {
+      a += __ldcg(ws + (size_t)g * C + c);
+      b += __ldcg(ws + ((size_t)G + g) * C + c);
+    }
+  }
+  tree_sum2<1>(&a, &b, fin.sub, fin.nc, fin.tpc);
+  if (fin.sub == 0 && c < C) {
+    // the coefficients of bwd_apply, from the same sums
+    const float is = invstd[c], db = a, dw = b * is, invM = 1.f / (float)M;
+    const float A = weight[c] * is;
+    s_A[fin.cl] = A;
+    s_D[fin.cl] = -A * is * (dw * invM);
+    s_E[fin.cl] = -A * (db * invM);
+    if (blockIdx.x == 0) {
+      dbias[c] = db;
+      dweight[c] = dw;
+    }
+  }
+  __syncthreads();
+  if (u >= units) return;
+
+  // phase 2
+  float A[kCh], D[kCh], E[kCh];
+#pragma unroll
+  for (int k = 0; k < kCh; ++k) {
+    A[k] = s_A[col * kCh + k];
+    D[k] = s_D[col * kCh + k];
+    E[k] = s_E[col * kCh + k];
+  }
+  const int ns = rows - nh;
+  for (int k = lane < ns ? (ns - 1 - lane) / RL : -1; k >= 0; k -= 2) {
+    const size_t i0 = (r0 + nh + lane + (size_t)k * RL) * units + u, i1 = i0 - (size_t)RL * units;
+    float d0[kCh], d1[kCh], f0[kCh], f1[kCh];
+    uint32_t b0 = 0, b1 = 0;
+    Unit<U>::load(dy, i0, d0);
+    Unit<U>::load(x, i0, f0);
+    if constexpr (kRelu) b0 = __ldcs(mask + i0);
+    if (k >= 1) {
+      Unit<U>::load(dy, i1, d1);
+      Unit<U>::load(x, i1, f1);
+      if constexpr (kRelu) b1 = __ldcs(mask + i1);
+    }
+    bwd_row<U, kRelu, kRes>(i0, mu, A, D, E, dx, dres, d0, f0, b0);
+    if (k >= 1) bwd_row<U, kRelu, kRes>(i1, mu, A, D, E, dx, dres, d1, f1, b1);
+  }
+  for (int j = lane; j < nh; j += RL) {
+    float d[kCh], f[kCh];
+    hold_load<U>(hdy + (j * CB + col) * V, d);
+    hold_load<U>(hx + (j * CB + col) * V, f);
+    bwd_row<U, kRelu, kRes>((r0 + j) * units + u, mu, A, D, E, dx, dres, d, f, kRelu ? hm[j * CB + col] : 0u);
+  }
+}
+
 // ---- synchronised batch norm: the cross-rank step between the local reduction and the apply pass -------------
 //
 // Window of one rank (float offsets from its base): slot (parity p, source rank r) at (p * W + r) * slot, with
@@ -566,6 +888,129 @@ int apply_grid(size_t M, const Geo& g, int per_sm) {
   return (int)(most < want ? (most < 1 ? 1 : most) : want);
 }
 
+// ---- single-launch host side
+constexpr int kMaxDevices = 64;
+
+int dtype_index(int dtype) { return dtype == WIRE_F32 ? 0 : dtype == WIRE_BF16 ? 1 : dtype == WIRE_F16 ? 2 : -1; }
+
+using FusedFwd = void (*)(const void*, const void*, size_t, int, int, size_t, int, float, float, float*, float*,
+                          float*, float*, const float*, const float*, void*, uint8_t*, float*, uint32_t*);
+using FusedBwd =void (*)(const void*, const void*, const uint8_t*, size_t, int, int, size_t, int, const float*,
+                          const float*, const float*, float*, float*, void*, void*, float*, uint32_t*);
+
+// Per device: the SM count and, per direction and dtype, the dynamic shared memory a block may hold when
+// kResBlocksPerSM blocks share an SM (0: the single-launch pass cannot run on this device).
+struct FusedDev {
+  int sms = 0;
+  size_t dyn[2][3] = {};
+};
+
+// Opts every variant of (direction, dtype) in to `*dyn` bytes of dynamic shared memory, first lowering *dyn by the
+// largest static shared memory of the variants; leaves *dyn = 0 unless each variant then fits kResBlocksPerSM blocks
+// per SM.
+template <class K>
+void opt_in(const K* kernels, int n, size_t share, size_t* dyn) {
+  size_t stat = 0;
+  for (int i = 0; i < n; ++i) {
+    cudaFuncAttributes a;
+    if (cudaFuncGetAttributes(&a, (const void*)kernels[i]) != cudaSuccess) return;
+    stat = a.sharedSizeBytes > stat ? a.sharedSizeBytes : stat;
+  }
+  if (share <= stat) return;
+  const size_t d = (share - stat) & ~(size_t)15;
+  for (int i = 0; i < n; ++i) {
+    int nb = 0;
+    if (cudaFuncSetAttribute((const void*)kernels[i], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)d) !=
+            cudaSuccess ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kernels[i], kT, d) != cudaSuccess || nb < kResBlocksPerSM)
+      return;
+  }
+  *dyn = d;
+}
+
+template <class U>
+void opt_in_u(size_t share, size_t* fwd, size_t* bwd) {
+  const FusedFwd f[4] = {bn_act_fwd_fused_kernel<U, false, false>, bn_act_fwd_fused_kernel<U, false, true>,
+                         bn_act_fwd_fused_kernel<U, true, false>, bn_act_fwd_fused_kernel<U, true, true>};
+  const FusedBwd b[4] = {bn_act_bwd_fused_kernel<U, false, false>, bn_act_bwd_fused_kernel<U, false, true>,
+                            bn_act_bwd_fused_kernel<U, true, false>, bn_act_bwd_fused_kernel<U, true, true>};
+  opt_in(f, 4, share, fwd);
+  opt_in(b, 4, share, bwd);
+}
+
+const FusedDev* fused_dev() {
+  static std::mutex mu;
+  static FusedDev devs[kMaxDevices];
+  static bool done[kMaxDevices] = {};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return nullptr;
+  std::lock_guard<std::mutex> lock(mu);
+  FusedDev& d = devs[dev];
+  if (!done[dev]) {
+    done[dev] = true;
+    int coop = 0, sms = 0, per_sm = 0, reserved = 0;
+    if (cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev) != cudaSuccess || !coop ||
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev) != cudaSuccess)
+      return &d;
+    const size_t share = (size_t)per_sm / kResBlocksPerSM - (size_t)reserved;
+    opt_in_u<TagF32>(share, &d.dyn[0][0], &d.dyn[1][0]);
+    opt_in_u<TagBF16>(share, &d.dyn[0][1], &d.dyn[1][1]);
+    opt_in_u<TagF16>(share, &d.dyn[0][2], &d.dyn[1][2]);
+    d.sms = sms;
+  }
+  return &d;
+}
+
+struct FusedPlan {
+  Geo g;
+  size_t rpc;   // rows per chunk, a multiple of RL
+  int G;        // chunks (gridDim.x)
+  int held;     // rows of a chunk held in shared memory: a multiple of RL, or rpc
+  size_t smem;  // dynamic shared memory per block
+};
+
+// Bytes of shared memory per held block row.
+size_t held_row_bytes(int bwd, int dtype, const Geo& g) {
+  const size_t vec = (size_t)kCh * (dtype == WIRE_F32 ? 4 : 2);
+  return ((size_t)1 << g.shift) * (bwd ? 2 * vec + 1 : vec);
+}
+
+bool fused_plan(int bwd, int dtype, size_t M, int C, long long cap, FusedPlan* p) {
+  const int dt = dtype_index(dtype);
+  const FusedDev* d = fused_dev();
+  if (dt < 0 || bad_shape(M, C) || d == nullptr || d->dyn[bwd ? 1 : 0][dt] == 0) return false;
+  const Geo g = geo(C, red_cb(C));
+  const int blocks = d->sms * kResBlocksPerSM;
+  if (g.ncb > blocks) return false;
+  const size_t want = (size_t)(blocks / g.ncb), rl = (size_t)g.rl;
+  size_t rpc = (M + want - 1) / want;
+  rpc = (rpc < rl ? rl : (rpc + rl - 1) / rl * rl);
+  size_t budget = d->dyn[bwd ? 1 : 0][dt];
+  if (cap >= 0 && (size_t)cap < budget) budget = (size_t)cap;
+  const size_t row = held_row_bytes(bwd, dtype, g);
+  size_t held = budget / row;
+  held = held >= rpc ? rpc : held / rl * rl;
+  *p = FusedPlan{g, rpc, (int)((M + rpc - 1) / rpc), (int)held, (held * row + 15) & ~(size_t)15};
+  return true;
+}
+
+template <class... P, class... A>
+cudaError_t launch_coop(void (*kernel)(P...), const FusedPlan& p, cudaStream_t s, A... args) {
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeCooperative;
+  attr[0].val.cooperative = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(p.G, p.g.ncb);
+  cfg.blockDim = dim3(kT);
+  cfg.dynamicSmemBytes = p.smem;
+  cfg.stream = s;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  return cudaLaunchKernelEx(&cfg, kernel, args...);
+}
+
 }  // namespace
 
 size_t bn_act_workspace_floats(size_t M, int C) {
@@ -649,6 +1094,45 @@ cudaError_t launch_bn_act_fwd_stats_local(const void* x, int dtype, size_t M, in
   return cudaGetLastError();
 }
 
+bool bn_act_fused_plan(int bwd, int dtype, size_t M, int C, long long cap, BnFusedPlan* out) {
+  FusedPlan p;
+  if (!fused_plan(bwd, dtype, M, C, cap, &p)) return false;
+  *out = BnFusedPlan{2 * (size_t)p.G * (size_t)C, p.g.ncb, p.rpc, p.held, p.smem, fused_dev()->sms * kResBlocksPerSM};
+  return true;
+}
+
+cudaError_t launch_bn_act_fwd(const void* x, const void* residual, int dtype, size_t M, int C, float eps,
+                              float momentum, float* running_mean, float* running_var, float* save_mean,
+                              float* save_invstd, const float* weight, const float* bias, int relu, void* y,
+                              uint8_t* mask, float* ws, uint32_t* counters, long long cap, cudaStream_t s) {
+  FusedPlan p;
+  if (bad_shape(M, C) || M < 2 || !aligned16(x) || !aligned16(residual) || !aligned16(y) ||
+      (relu && mask == nullptr) || (running_mean == nullptr) != (running_var == nullptr))
+    return cudaErrorInvalidValue;
+  if (!fused_plan(0, dtype, M, C, cap, &p)) return cudaErrorNotSupported;
+  cudaError_t e = cudaSuccess;
+  BN_DISPATCH_U(dtype, BN_DISPATCH_B(relu, kRelu, BN_DISPATCH_B(residual != nullptr, kRes, (
+      e = launch_coop(bn_act_fwd_fused_kernel<U, kRelu, kRes>, p, s, x, residual, M, C, p.g.shift, p.rpc, p.held,
+                         eps, momentum, running_mean, running_var, save_mean, save_invstd, weight, bias, y, mask, ws,
+                         counters)))));
+  return e;
+}
+
+cudaError_t launch_bn_act_bwd(const void* dy, const void* x, const uint8_t* mask, int dtype, size_t M, int C,
+                              const float* mean, const float* invstd, const float* weight, float* dweight,
+                              float* dbias, void* dx, void* dresidual, float* ws, uint32_t* counters, long long cap,
+                              cudaStream_t s) {
+  FusedPlan p;
+  if (bad_shape(M, C) || !aligned16(dy) || !aligned16(x) || !aligned16(dx) || !aligned16(dresidual))
+    return cudaErrorInvalidValue;
+  if (!fused_plan(1, dtype, M, C, cap, &p)) return cudaErrorNotSupported;
+  cudaError_t e = cudaSuccess;
+  BN_DISPATCH_U(dtype, BN_DISPATCH_B(mask != nullptr, kRelu, BN_DISPATCH_B(dresidual != nullptr, kRes, (
+      e = launch_coop(bn_act_bwd_fused_kernel<U, kRelu, kRes>, p, s, dy, x, mask, M, C, p.g.shift, p.rpc, p.held,
+                      mean, invstd, weight, dweight, dbias, dx, dresidual, ws, counters)))));
+  return e;
+}
+
 size_t bn_sync_window_floats(int world, int cmax) { return 2 * (size_t)world * (kSyncPad + 2 * (size_t)cmax); }
 
 namespace {
@@ -723,6 +1207,7 @@ cudaError_t bn_act_load_kernels() {
   if (e == cudaSuccess) e = load_u<TagF16>();
   if (e == cudaSuccess) e = load1(bn_sync_kernel<true>);
   if (e == cudaSuccess) e = load1(bn_sync_kernel<false>);
+  if (e == cudaSuccess && fused_dev() == nullptr) e = cudaErrorInvalidDevice;
   return e;
 }
 

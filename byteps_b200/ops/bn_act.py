@@ -2,9 +2,10 @@
 
 ``BatchNormAct2d`` is an ``nn.BatchNorm2d`` (same parameters, buffers and state_dict keys) whose
 ``forward(x, residual=None)`` computes ``act(batch_norm(x) [+ residual])``.  On a CUDA, NHWC-contiguous
-(channels_last) input in training mode it runs two sm_90a kernels forward (statistics, then apply + 1-bit ReLU
-mask) and two backward (reduce, then apply), instead of torch's separate batch-norm, add, ReLU and
-threshold-backward passes.  Every other input - CPU, eval mode, NCHW, C not a multiple of 8 - takes the stock
+(channels_last) input in training mode it runs one sm_90a kernel forward (statistics, grid barrier, apply + 1-bit
+ReLU mask) and one backward (reduce, grid barrier, apply), or two each (the same phases as separate launches) where
+the device cannot run the single-launch kernels at that shape, instead of torch's separate batch-norm, add, ReLU
+and threshold-backward passes.  Every other input - CPU, eval mode, NCHW, C not a multiple of 8 - takes the stock
 ``F.batch_norm`` / add / ``relu`` composition, which computes the same function.
 """
 from __future__ import annotations
@@ -30,7 +31,24 @@ def _nhwc(t: torch.Tensor) -> bool:
     return t.is_contiguous(memory_format=torch.channels_last)
 
 
+#: Bytes of rows a block of the single-launch kernels may hold in shared memory; None: as many as fit.  Only tests
+#: change it, to reach the fully held, partly held and fully streamed (0) cases at small shapes.
+RESIDENT_CAP: Optional[int] = None
+
+
+def _cap() -> int:
+    return -1 if RESIDENT_CAP is None else int(RESIDENT_CAP)
+
+
+def _workspace(nws, nctr, device):
+    return (torch.empty(nws, dtype=torch.float32, device=device),
+            torch.zeros(nctr, dtype=torch.int32, device=device))
+
+
 class _BatchNormActFn(torch.autograd.Function):
+    """Each direction is one single-launch kernel where the device can run it at the input's shape
+    (``bn_act_plan``), and the two-pass kernels otherwise."""
+
     @staticmethod
     def forward(ctx, x, residual, weight, bias, running_mean, running_var, momentum, eps, relu):
         cu = _native.cuda()
@@ -40,17 +58,24 @@ class _BatchNormActFn(torch.autograd.Function):
         stream = torch.cuda.current_stream(x.device).cuda_stream
         f32 = dict(dtype=torch.float32, device=x.device)
         mean, invstd = torch.empty(c, **f32), torch.empty(c, **f32)
-        nws, nctr = cu.bn_act_workspace(m, c)
-        ws = torch.empty(nws, **f32)
-        ctr = torch.zeros(nctr, dtype=torch.int32, device=x.device)
-        cu.bn_act_fwd_stats(x.data_ptr(), code, m, c, float(eps), float(momentum), _ptr(running_mean),
-                            _ptr(running_var), mean.data_ptr(), invstd.data_ptr(), ws.data_ptr(), ctr.data_ptr(), stream)
         y = torch.empty_like(x)
         mask = torch.empty((m, c // _UNIT), dtype=torch.uint8, device=x.device) if relu else None
-        cu.bn_act_fwd_apply(x.data_ptr(), _ptr(residual), code, m, c, mean.data_ptr(), invstd.data_ptr(),
-                            weight.data_ptr(), bias.data_ptr(), bool(relu), y.data_ptr(), _ptr(mask), stream)
+        plan = cu.bn_act_plan(0, code, m, c, _cap())
+        if plan is not None:
+            ws, ctr = _workspace(plan["ws_floats"], plan["counters"], x.device)
+            cu.bn_act_fwd(x.data_ptr(), _ptr(residual), code, m, c, float(eps), float(momentum), _ptr(running_mean),
+                          _ptr(running_var), mean.data_ptr(), invstd.data_ptr(), weight.data_ptr(), bias.data_ptr(),
+                          bool(relu), y.data_ptr(), _ptr(mask), ws.data_ptr(), ctr.data_ptr(), stream, _cap())
+        else:
+            ws, ctr = _workspace(*cu.bn_act_workspace(m, c), x.device)
+            cu.bn_act_fwd_stats(x.data_ptr(), code, m, c, float(eps), float(momentum), _ptr(running_mean),
+                                _ptr(running_var), mean.data_ptr(), invstd.data_ptr(), ws.data_ptr(), ctr.data_ptr(),
+                                stream)
+            cu.bn_act_fwd_apply(x.data_ptr(), _ptr(residual), code, m, c, mean.data_ptr(), invstd.data_ptr(),
+                                weight.data_ptr(), bias.data_ptr(), bool(relu), y.data_ptr(), _ptr(mask), stream)
         ctx.save_for_backward(x, weight, mean, invstd, mask)
         ctx.has_residual = residual is not None
+        ctx.single_launch_fwd = plan is not None
         return y
 
     @staticmethod
@@ -64,15 +89,22 @@ class _BatchNormActFn(torch.autograd.Function):
         stream = torch.cuda.current_stream(x.device).cuda_stream
         f32 = dict(dtype=torch.float32, device=x.device)
         dweight, dbias = torch.empty(c, **f32), torch.empty(c, **f32)
-        nws, nctr = cu.bn_act_workspace(m, c)
-        ws = torch.empty(nws, **f32)
-        ctr = torch.zeros(nctr, dtype=torch.int32, device=x.device)
-        cu.bn_act_bwd_reduce(dy.data_ptr(), x.data_ptr(), _ptr(mask), code, m, c, mean.data_ptr(), invstd.data_ptr(),
-                             dweight.data_ptr(), dbias.data_ptr(), ws.data_ptr(), ctr.data_ptr(), stream)
         dx = torch.empty_like(x)
         dres = torch.empty_like(x) if ctx.has_residual else None
-        cu.bn_act_bwd_apply(dy.data_ptr(), x.data_ptr(), _ptr(mask), code, m, c, mean.data_ptr(), invstd.data_ptr(),
-                            weight.data_ptr(), dweight.data_ptr(), dbias.data_ptr(), dx.data_ptr(), _ptr(dres), stream)
+        plan = cu.bn_act_plan(1, code, m, c, _cap())
+        if plan is not None:
+            ws, ctr = _workspace(plan["ws_floats"], plan["counters"], x.device)
+            cu.bn_act_bwd(dy.data_ptr(), x.data_ptr(), _ptr(mask), code, m, c, mean.data_ptr(), invstd.data_ptr(),
+                          weight.data_ptr(), dweight.data_ptr(), dbias.data_ptr(), dx.data_ptr(), _ptr(dres),
+                          ws.data_ptr(), ctr.data_ptr(), stream, _cap())
+        else:
+            ws, ctr = _workspace(*cu.bn_act_workspace(m, c), x.device)
+            cu.bn_act_bwd_reduce(dy.data_ptr(), x.data_ptr(), _ptr(mask), code, m, c, mean.data_ptr(),
+                                 invstd.data_ptr(), dweight.data_ptr(), dbias.data_ptr(), ws.data_ptr(), ctr.data_ptr(),
+                                 stream)
+            cu.bn_act_bwd_apply(dy.data_ptr(), x.data_ptr(), _ptr(mask), code, m, c, mean.data_ptr(),
+                                invstd.data_ptr(), weight.data_ptr(), dweight.data_ptr(), dbias.data_ptr(),
+                                dx.data_ptr(), _ptr(dres), stream)
         return dx, dres, dweight, dbias, None, None, None, None, None
 
 
