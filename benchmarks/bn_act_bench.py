@@ -16,7 +16,9 @@ are the least each fused pass must move, computed from the shape (e = element by
     single:bwd  read dy, x [, mask] once; write dx [, dres]  N e (3 [+1]) [+ N / 8]   (bwd_reduce + bwd_apply)
 
 The fused:fwd / fused:bwd rows sum the two-pass kernels; the single rows are the single-launch kernels the module
-takes where their plan allows it.  Every timed launch moves to the next of enough copies of the tensors that the
+takes where their plan allows it.  Those rows also print the bytes the launch actually moves (the plan's
+bytes_moved: the rows a block does not hold are read twice) with the share of peak over them, and the plan's held
+rows per chunk and ring depth.  Every timed launch moves to the next of enough copies of the tensors that the
 launches of a row touch more than --rotate-mb together, so no pass finds its input in the 50 MB L2 from the launch
 before.  The stock rows time F.batch_norm [+ add] [+ relu] and its autograd backward; their GB/s use the fused passes'
 bytes, i.e. they are the rate at which the stock sequence delivers the same work.  Share of peak is against the
@@ -86,7 +88,8 @@ def main():
     info = gpu_info()
     rows = []
     print("GPU: %s; batch %d, bf16 activations, fp32 parameters, NHWC" % (info, args.batch))
-    print("%-14s %-9s %-11s %9s %9s %8s %6s" % ("C x H x W", "variant", "pass", "MB", "us", "GB/s", "%peak"))
+    print("%-14s %-9s %-11s %9s %9s %8s %6s %9s %7s" % ("C x H x W", "variant", "pass", "MB", "us", "GB/s", "%peak",
+                                                       "moved MB", "%peak"))
     for (c, h, w) in SHAPES:
         variants = ["relu"] + (["relu_res", "none"] if (c, h, w) in EXPANDED else [])
         n, m = args.batch * c * h * w, args.batch * h * w
@@ -137,7 +140,8 @@ def main():
                 rows.append(dict(shape=[c, h, w], variant=var, impl="fused", kind=name, bytes=nbytes, us=ms * 1e3))
 
             # the single-launch kernels; their counters are left non-zero, so each launch gets a zeroed set
-            fplan, bplan = cu.bn_act_plan(0, code, m, c), cu.bn_act_plan(1, code, m, c)
+            fplan = cu.bn_act_plan(0, code, m, c, relu=relu, residual=res)
+            bplan = cu.bn_act_plan(1, code, m, c, relu=relu, residual=res)
             single = []
             if fplan is not None and bplan is not None:
                 nctr1 = max(fplan["counters"], bplan["counters"])
@@ -163,9 +167,10 @@ def main():
                     launch[0] = 0
                     ctrs.zero_()
                     ms = timed(fn, k)
+                    plan = fplan if name == "fwd" else bplan
                     rows.append(dict(shape=[c, h, w], variant=var, impl="single", kind=name, bytes=nbytes,
-                                     us=ms * 1e3, held_rows=(fplan if name == "fwd" else bplan)["held_rows"],
-                                     rows_per_chunk=fplan["rows_per_chunk"]))
+                                     us=ms * 1e3, held_rows=plan["held_rows"], rows_per_chunk=plan["rows_per_chunk"],
+                                     ring_depth=plan["ring_depth"], bytes_moved=plan["bytes_moved"]))
 
             # stock sequence on the same tensors
             XS = [t["x"].detach().requires_grad_(True) for t in T]
@@ -195,9 +200,15 @@ def main():
             for row in rows[-(len(passes) + len(single) + 4):]:
                 gbs = row["bytes"] / (row["us"] * 1e3)
                 row["gbs"], row["peak_share"] = gbs, gbs / PEAK_GBS
-                print("%-14s %-9s %-11s %9.1f %9.1f %8.0f %5.0f%%" % (
+                extra = ""
+                if row["impl"] == "single":
+                    row["moved_share"] = row["bytes_moved"] / (row["us"] * 1e3) / PEAK_GBS
+                    extra = " %9.1f %6.0f%%  held %d/%d ring %d" % (
+                        row["bytes_moved"] / 1e6, 100 * row["moved_share"], row["held_rows"], row["rows_per_chunk"],
+                        row["ring_depth"])
+                print("%-14s %-9s %-11s %9.1f %9.1f %8.0f %5.0f%%%s" % (
                     "%dx%dx%d" % (c, h, w), var, row["impl"] + ":" + row["kind"], row["bytes"] / 1e6, row["us"], gbs,
-                    100 * row["peak_share"]))
+                    100 * row["peak_share"], extra))
             del T, P, XS, RS
     f_tot = sum(r_["us"] for r_ in rows if r_["impl"] == "fused" and r_["kind"] in ("fwd", "bwd"))
     g_tot = sum(r_["us"] for r_ in rows if r_["impl"] == "single")

@@ -60,20 +60,25 @@ void bind_cuda_bn(py::module_& m) {
      "total: device float holding the row count to divide by (bn_sync_stats writes it); 0 divides by M");
 
   // ---- single-launch passes
-  m.def("bn_act_plan", [](int bwd, int dtype, size_t M, int C, long long cap) -> py::object {
+  m.def("bn_act_plan", [](int bwd, int dtype, size_t M, int C, long long cap, bool relu, bool residual) -> py::object {
     BnFusedPlan p;
-    if (!bn_act_fused_plan(bwd, dtype, M, C, cap, &p)) return py::none();
+    if (!bn_act_fused_plan(bwd, dtype, M, C, cap, relu ? 1 : 0, residual ? 1 : 0, &p)) return py::none();
     py::dict d;
     d["ws_floats"] = p.ws_floats;
     d["counters"] = p.counters;
     d["rows_per_chunk"] = p.rows_per_chunk;
     d["held_rows"] = p.held_rows;
     d["held_bytes"] = p.held_bytes;
+    d["ring_depth"] = p.ring_depth;
+    d["smem_bytes"] = p.smem_bytes;
+    d["bytes_moved"] = p.bytes_moved;
     d["wave_blocks"] = p.wave_blocks;
     return d;
-  }, py::arg("bwd"), py::arg("dtype"), py::arg("M"), py::arg("C"), py::arg("cap") = -1,
+  }, py::arg("bwd"), py::arg("dtype"), py::arg("M"), py::arg("C"), py::arg("cap") = -1, py::arg("relu") = false,
+     py::arg("residual") = false,
      "plan of the single-launch bn_act_fwd (bwd=0) / bn_act_bwd (bwd=1) at (M, C, dtype) on the current device, or "
-     "None when it cannot run there; cap >= 0 limits the bytes of rows a block holds in shared memory");
+     "None when it cannot run there; cap >= 0 limits the bytes of rows a block holds in shared memory.  relu and "
+     "residual only select the variant whose bytes_moved is reported");
   m.def("bn_act_fwd", [](uintptr_t x, uintptr_t residual, int dtype, size_t M, int C, float eps, float momentum,
                          uintptr_t running_mean, uintptr_t running_var, uintptr_t save_mean, uintptr_t save_invstd,
                          uintptr_t weight, uintptr_t bias, bool relu, uintptr_t y, uintptr_t mask, uintptr_t ws,

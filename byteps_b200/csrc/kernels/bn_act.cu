@@ -111,60 +111,93 @@ __device__ __forceinline__ void chan_merge(float& n, float* mean, float* m2, flo
   n = nn;
 }
 
-// Fixed-order tree over the `lanes` threads of a column: thread t = lane * cols + col (t == threadIdx.x);
-// the result is in lane 0.
+// Fixed-order tree over the `lanes` threads of a column: thread t = lane * cols + col (t == threadIdx.x,
+// lanes * cols == kT); the result is in lane 0.  At level s lane L < s takes lane L + s, i.e. thread t + s * cols.
+// The levels with s * cols >= 32 pair threads of different warps and go through shared memory, where the senders
+// t in [s * cols, 2 s * cols) need only kT / 2 slots; the rest pair threads of warp 0 and use shuffles.
 template <int K>
 __device__ __forceinline__ void tree_welford(float& n, float* mean, float* m2, int lane, int cols, int lanes) {
-  __shared__ float sh[2 * K + 1][kT];
+  __shared__ float sh[2 * K + 1][kT / 2];
   const int t = threadIdx.x;
-  for (int s = lanes >> 1; s >= 1; s >>= 1) {
+  int s = lanes >> 1;
+  for (; s * cols >= 32; s >>= 1) {
     __syncthreads();
     if (lane >= s && lane < 2 * s) {
-      sh[0][t] = n;
+      const int p = t - s * cols;
+      sh[0][p] = n;
 #pragma unroll
       for (int k = 0; k < K; ++k) {
-        sh[1 + k][t] = mean[k];
-        sh[1 + K + k][t] = m2[k];
+        sh[1 + k][p] = mean[k];
+        sh[1 + K + k][p] = m2[k];
       }
     }
     __syncthreads();
     if (lane < s) {
-      const int p = t + s * cols;
       float mb[K], m2b[K];
 #pragma unroll
       for (int k = 0; k < K; ++k) {
-        mb[k] = sh[1 + k][p];
-        m2b[k] = sh[1 + K + k][p];
+        mb[k] = sh[1 + k][t];
+        m2b[k] = sh[1 + K + k][t];
       }
-      chan_merge<K>(n, mean, m2, sh[0][p], mb, m2b);
+      chan_merge<K>(n, mean, m2, sh[0][t], mb, m2b);
+    }
+  }
+  if (t < 32) {
+    for (; s >= 1; s >>= 1) {
+      const int d = s * cols;
+      const float nb = __shfl_down_sync(0xffffffffu, n, d);
+      float mb[K], m2b[K];
+#pragma unroll
+      for (int k = 0; k < K; ++k) {
+        mb[k] = __shfl_down_sync(0xffffffffu, mean[k], d);
+        m2b[k] = __shfl_down_sync(0xffffffffu, m2[k], d);
+      }
+      if (lane < s) chan_merge<K>(n, mean, m2, nb, mb, m2b);
     }
   }
 }
 
+// The same tree as tree_welford, adding two K-vectors.
 template <int K>
 __device__ __forceinline__ void tree_sum2(float* a, float* b, int lane, int cols, int lanes) {
-  __shared__ float sh[2 * K][kT];
+  __shared__ float sh[2 * K][kT / 2];
   const int t = threadIdx.x;
-  for (int s = lanes >> 1; s >= 1; s >>= 1) {
+  int s = lanes >> 1;
+  for (; s * cols >= 32; s >>= 1) {
     __syncthreads();
     if (lane >= s && lane < 2 * s) {
+      const int p = t - s * cols;
 #pragma unroll
       for (int k = 0; k < K; ++k) {
-        sh[k][t] = a[k];
-        sh[K + k][t] = b[k];
+        sh[k][p] = a[k];
+        sh[K + k][p] = b[k];
       }
     }
     __syncthreads();
     if (lane < s) {
-      const int p = t + s * cols;
 #pragma unroll
       for (int k = 0; k < K; ++k) {
-        a[k] += sh[k][p];
-        b[k] += sh[K + k][p];
+        a[k] += sh[k][t];
+        b[k] += sh[K + k][t];
+      }
+    }
+  }
+  if (t < 32) {
+    for (; s >= 1; s >>= 1) {
+      const int d = s * cols;
+#pragma unroll
+      for (int k = 0; k < K; ++k) {
+        const float ab = __shfl_down_sync(0xffffffffu, a[k], d), bb = __shfl_down_sync(0xffffffffu, b[k], d);
+        if (lane < s) {
+          a[k] += ab;
+          b[k] += bb;
+        }
       }
     }
   }
 }
+
+constexpr int kMaxRedCh = 8 * kCh;   // channels of a reduction-layout channel group (red_cb <= 8 units)
 
 // Finalize layout of the last block of a channel group: nc = CB * kCh channels, tpc = kT / nc threads per channel
 // (thread t: channel t % nc, lane t / nc).  Each lane sums a fixed stride of the G chunk partials, then a fixed
@@ -174,7 +207,7 @@ struct Fin {
   __device__ Fin(int CB) : nc(CB * kCh), tpc(kT / (CB * kCh)), cl(threadIdx.x % (CB * kCh)),
                            sub(threadIdx.x / (CB * kCh)) {}
   __device__ float all_sum(float v) const {
-    __shared__ float out[kT];
+    __shared__ float out[kMaxRedCh];
     float dummy = 0.f;
     tree_sum2<1>(&v, &dummy, sub, nc, tpc);
     __syncthreads();
@@ -478,8 +511,20 @@ __global__ void __launch_bounds__(kT, kBwdApplyBlocksPerSM) bn_act_bwd_apply_ker
 // that what phase 1 read last, the part most likely still in L2, is read first.  Between the phases every block of a
 // channel group waits for the group's partials and merges them itself, in the same fixed order, so all of the group's
 // blocks get the same bits without a second barrier.
+//
+// Streamed rows pass through a ring of kStages[bwd] block row-steps in shared memory behind the held rows, fed by
+// cp.async: one commit group per row-step, and a thread only ever reads the slots it filled itself, so the ring needs
+// no block synchronisation.  Phase 1 pushes a thread's rows in row order (held rows first, as they come first in the
+// chunk), so the statistics do not depend on how many rows are held.
+//
+// Shared memory of a block, in units of one row-step (kT threads x one unit: kT * V Vec16) with the thread's slot at
+// t * V inside it:
+//   forward    x of held / RL steps | ring: kFwdStages steps of x (with a residual, phase 2 pairs them: x, residual)
+//   backward   dy of held / RL steps | x of them | their mask words | ring: kBwdStages x (dy step, x step, mask words)
+// A mask word is the aligned 4-byte word holding the thread's mask byte (mask_copy).
 constexpr int kResBlocksPerSM = 2;
-constexpr int kMaxRedCh = 8 * kCh;   // channels of a reduction-layout channel group (red_cb <= 8 units)
+constexpr int kFwdStages = 4;
+constexpr int kBwdStages = 2;
 
 __device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
   uint32_t v;
@@ -489,7 +534,49 @@ __device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
 __device__ __forceinline__ void cp_async16(void* smem, const void* g) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem)), "l"(g) : "memory");
 }
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+__device__ __forceinline__ void cp_async4(void* smem, const void* g) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(smem)), "l"(g) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+
+// Copies the aligned 4-byte word holding mask byte i to *w; mask_byte extracts the byte again.  A word reaching
+// outside the n mask bytes (at most the first and the last) is assembled from the byte alone.
+__device__ __forceinline__ void mask_copy(uint32_t* w, const uint8_t* mask, size_t i, size_t n) {
+  const uintptr_t a = (uintptr_t)(mask + i), a0 = a & ~(uintptr_t)3;
+  if (a0 >= (uintptr_t)mask && a0 + 4 <= (uintptr_t)(mask + n))
+    cp_async4(w, reinterpret_cast<const void*>(a0));
+  else
+    *w = (uint32_t)mask[i] << (8 * (a & 3));
+}
+__device__ __forceinline__ uint32_t mask_byte(uint32_t w, const uint8_t* mask, size_t i) {
+  return (w >> (8 * (((uintptr_t)mask + i) & 3))) & 0xffu;
+}
+
+// Runs use(k, slot) for k = 0 .. n - 1 with the copies of step k, started by issue(k, slot), complete: D steps in
+// flight, step k in ring slot k % D.  The groups of steps 0 .. D - 1 are the last D the thread committed
+// (ring_fill); groups committed before them complete first.
+template <int D, class Issue, class Use>
+__device__ __forceinline__ void ring_drain(int n, Issue issue, Use use) {
+  for (int k = 0; k < n; ++k) {
+    cp_async_wait<D - 1>();
+    const int slot = k % D;
+    use(k, slot);
+    if (k + D < n) issue(k + D, slot);
+    cp_async_commit();
+  }
+}
+template <int D, class Issue>
+__device__ __forceinline__ void ring_fill(int n, Issue issue) {
+#pragma unroll 1
+  for (int k = 0; k < D; ++k) {
+    if (k < n) issue(k, k);
+    cp_async_commit();
+  }
+}
 
 // One-shot barrier of the gridDim.x blocks of a channel group on a zeroed counter.  Only cooperative launches use
 // it, so every block is resident and the wait ends; the time limit turns a broken launch into an error, not a hang.
@@ -521,46 +608,47 @@ __device__ __forceinline__ void hold_copy(Vec16* h, const void* base, size_t uni
   for (int v = 0; v < Unit<U>::kVecs; ++v) cp_async16(h + v, p + v);
 }
 
-// Dynamic shared memory: x of `held` block rows, CB units each.
+// Dynamic shared memory: x of `held` block rows, then the ring (see above).
 template <class U, bool kRelu, bool kRes>
 __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_fwd_fused_kernel(
     const void* __restrict__ x, const void* __restrict__ res, size_t M, int C, int shift, size_t rpc, int held,
     float eps, float momentum, float* run_mean, float* run_var, float* save_mean, float* save_invstd,
     const float* weight, const float* bias, void* y, uint8_t* mask, float* ws, uint32_t* counters) {
   extern __shared__ Vec16 hold[];
-  constexpr int V = Unit<U>::kVecs;
+  constexpr int V = Unit<U>::kVecs, SV = kT * V;   // SV: Vec16 of one row-step
   __shared__ float s_mu[kMaxRedCh], s_sc[kMaxRedCh];
   const int units = C / kCh, CB = 1 << shift, RL = kT >> shift;
   const int col = threadIdx.x & (CB - 1), lane = threadIdx.x >> shift;
   const int u = blockIdx.y * CB + col;
   const size_t r0 = (size_t)blockIdx.x * rpc, r1 = min(M, r0 + rpc);
   const int rows = (int)(r1 - r0), nh = min(held, rows);
+  // this thread's held and streamed rows (row-steps), their first units and the units between two of them
+  const int hn = lane < nh ? (nh - 1 - lane) / RL + 1 : 0;
+  const int sn = lane < rows - nh ? (rows - nh - 1 - lane) / RL + 1 : 0;
+  const size_t i_h = (r0 + lane) * units + u, i_s = i_h + (size_t)nh * units, ustep = (size_t)RL * units;
+  Vec16* hx = hold + threadIdx.x * V;                                  // held step k at hx + k * SV
+  Vec16* ring = hold + (size_t)(held / RL) * SV + threadIdx.x * V;     // ring slot j at ring + j * SV
 
-  // phase 1: held rows to shared memory, streamed rows through registers; Welford over all of them
+  // phase 1: Welford over the thread's rows in row order, the held ones copied to shared memory on the way
   float n = 0.f, mean[kCh], m2[kCh];
 #pragma unroll
   for (int k = 0; k < kCh; ++k) mean[k] = m2[k] = 0.f;
   if (u < units) {
-    for (int j = lane; j < nh; j += RL) hold_copy<U>(hold + (j * CB + col) * V, x, (r0 + j) * units + u);
-    size_t r = r0 + nh + lane;
-    for (; r + 3 * RL < r1; r += 4 * RL) {
-      float f[4][kCh];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) Unit<U>::load(x, (r + j * RL) * units + u, f[j]);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) welford_push(n, mean, m2, f[j]);
-    }
-    for (; r < r1; r += RL) {
+    for (int k = 0; k < hn; ++k) hold_copy<U>(hx + (size_t)k * SV, x, i_h + k * ustep);
+    cp_async_commit();
+    auto issue = [&](int k, int slot) { hold_copy<U>(ring + slot * SV, x, i_s + k * ustep); };
+    ring_fill<kFwdStages>(sn, issue);
+    cp_async_wait<kFwdStages>();
+    for (int k = 0; k < hn; ++k) {
       float f[kCh];
-      Unit<U>::load(x, r * units + u, f);
+      hold_load<U>(hx + (size_t)k * SV, f);
       welford_push(n, mean, m2, f);
     }
-    cp_async_wait_all();
-    for (int j = lane; j < nh; j += RL) {
+    ring_drain<kFwdStages>(sn, issue, [&](int, int slot) {
       float f[kCh];
-      hold_load<U>(hold + (j * CB + col) * V, f);
+      hold_load<U>(ring + slot * SV, f);
       welford_push(n, mean, m2, f);
-    }
+    });
   }
   tree_welford<kCh>(n, mean, m2, lane, CB, RL);
   const int G = gridDim.x;
@@ -593,7 +681,9 @@ __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_fwd_fused_kernel(
   __syncthreads();
   if (u >= units) return;
 
-  // phase 2: streamed rows, last read first, then the held rows
+  // phase 2: streamed rows, last read first, then the held rows.  The ring carries x of the streamed rows and, with
+  // a residual, the residual of every row, in pairs of slots.  A block holding its whole chunk has no ring and reads
+  // the residual directly.
   float mu[kCh], sc[kCh], sh[kCh];
 #pragma unroll
   for (int k = 0; k < kCh; ++k) {
@@ -601,112 +691,106 @@ __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_fwd_fused_kernel(
     sc[k] = s_sc[col * kCh + k];
     sh[k] = bias[u * kCh + k];
   }
-  const int ns = rows - nh;
-  for (int k = lane < ns ? (ns - 1 - lane) / RL : -1; k >= 0; k -= 2) {
-    const size_t i0 = (r0 + nh + lane + (size_t)k * RL) * units + u, i1 = i0 - (size_t)RL * units;
-    float f0[kCh], f1[kCh], q0[kCh], q1[kCh];
-    Unit<U>::load(x, i0, f0);
-    if constexpr (kRes) Unit<U>::load(res, i0, q0);
-    if (k >= 1) {
-      Unit<U>::load(x, i1, f1);
-      if constexpr (kRes) Unit<U>::load(res, i1, q1);
-    }
-    fwd_row<U, kRelu, kRes>(i0, mu, sc, sh, y, mask, f0, q0);
-    if (k >= 1) fwd_row<U, kRelu, kRes>(i1, mu, sc, sh, y, mask, f1, q1);
-  }
-  for (int j = lane; j < nh; j += 2 * RL) {
-    const size_t i0 = (r0 + j) * units + u, i1 = i0 + (size_t)RL * units;
-    const bool two = j + RL < nh;
+  constexpr int W = kRes ? 2 : 1, D2 = kFwdStages / W;
+  const int n2 = sn + (kRes && (size_t)held < rpc ? hn : 0);
+  auto unit2 = [&](int k) { return k < sn ? i_s + (size_t)(sn - 1 - k) * ustep : i_h + (size_t)(k - sn) * ustep; };
+  auto issue2 = [&](int k, int slot) {
+    const size_t i = unit2(k);
+    if (k < sn) hold_copy<U>(ring + slot * W * SV, x, i);
+    if constexpr (kRes) hold_copy<U>(ring + (slot * W + 1) * SV, res, i);
+  };
+  ring_fill<D2>(n2, issue2);
+  ring_drain<D2>(n2, issue2, [&](int k, int slot) {
+    float f[kCh], q[kCh];
+    hold_load<U>(k < sn ? ring + slot * W * SV : hx + (size_t)(k - sn) * SV, f);
+    if constexpr (kRes) hold_load<U>(ring + (slot * W + 1) * SV, q);
+    fwd_row<U, kRelu, kRes>(unit2(k), mu, sc, sh, y, mask, f, q);
+  });
+  for (int k = n2 - sn; k < hn; k += 2) {   // the held rows the ring did not carry
+    const size_t i0 = i_h + k * ustep, i1 = i0 + ustep;
+    const bool two = k + 1 < hn;
     float f0[kCh], f1[kCh], q0[kCh], q1[kCh];
     if constexpr (kRes) {
       Unit<U>::load(res, i0, q0);
       if (two) Unit<U>::load(res, i1, q1);
     }
-    hold_load<U>(hold + (j * CB + col) * V, f0);
+    hold_load<U>(hx + (size_t)k * SV, f0);
     fwd_row<U, kRelu, kRes>(i0, mu, sc, sh, y, mask, f0, q0);
     if (two) {
-      hold_load<U>(hold + ((j + RL) * CB + col) * V, f1);
+      hold_load<U>(hx + (size_t)(k + 1) * SV, f1);
       fwd_row<U, kRelu, kRes>(i1, mu, sc, sh, y, mask, f1, q1);
     }
   }
 }
 
-// Dynamic shared memory: dy, then x of `held` block rows (CB units each), then their mask bytes.
+// Dynamic shared memory: dy, x and the mask words of `held` block rows, then the ring (see above).
 template <class U, bool kRelu, bool kRes>
 __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_bwd_fused_kernel(
     const void* __restrict__ dy, const void* __restrict__ x, const uint8_t* __restrict__ mask, size_t M, int C,
     int shift, size_t rpc, int held, const float* mean, const float* invstd, const float* weight, float* dweight,
     float* dbias, void* dx, void* dres, float* ws, uint32_t* counters) {
   extern __shared__ Vec16 hold[];
-  constexpr int V = Unit<U>::kVecs;
+  // SV: Vec16 of one row-step of dy or x; RS: of one ring slot (dy, x, then kT mask words)
+  constexpr int V = Unit<U>::kVecs, SV = kT * V, RS = 2 * SV + kT / 4;
   __shared__ float s_A[kMaxRedCh], s_D[kMaxRedCh], s_E[kMaxRedCh];
   const int units = C / kCh, CB = 1 << shift, RL = kT >> shift;
   const int col = threadIdx.x & (CB - 1), lane = threadIdx.x >> shift;
   const int u = blockIdx.y * CB + col;
   const size_t r0 = (size_t)blockIdx.x * rpc, r1 = min(M, r0 + rpc);
   const int rows = (int)(r1 - r0), nh = min(held, rows);
-  Vec16* hdy = hold;
-  Vec16* hx = hold + (size_t)held * CB * V;
-  uint8_t* hm = reinterpret_cast<uint8_t*>(hx + (size_t)held * CB * V);
+  const int hn = lane < nh ? (nh - 1 - lane) / RL + 1 : 0;
+  const int sn = lane < rows - nh ? (rows - nh - 1 - lane) / RL + 1 : 0;
+  const size_t i_h = (r0 + lane) * units + u, i_s = i_h + (size_t)nh * units, ustep = (size_t)RL * units;
+  const size_t nm = M * units;
+  const int t = threadIdx.x;
+  const size_t hs = (size_t)(held / RL);
+  Vec16* hdy = hold + t * V;                                            // held step k at hdy + k * SV, x likewise
+  Vec16* hx = hdy + hs * SV;
+  uint32_t* hm = reinterpret_cast<uint32_t*>(hold + 2 * hs * SV) + t;   // its mask word at hm + k * kT
+  Vec16* ring = hold + hs * (2 * SV + kT / 4);                          // ring slot j at ring + j * RS
+  auto slot_dy = [&](int j) { return ring + j * RS + t * V; };
+  auto slot_x = [&](int j) { return ring + j * RS + SV + t * V; };
+  auto slot_m = [&](int j) { return reinterpret_cast<uint32_t*>(ring + j * RS + 2 * SV) + t; };
+  auto issue_at = [&](int j, size_t i) {
+    hold_copy<U>(slot_dy(j), dy, i);
+    hold_copy<U>(slot_x(j), x, i);
+    if constexpr (kRelu) mask_copy(slot_m(j), mask, i, nm);
+  };
 
-  // phase 1
+  // phase 1: the thread's rows in row order, the held ones copied to shared memory on the way
   float sg[kCh], sgx[kCh], mu[kCh];
 #pragma unroll
   for (int k = 0; k < kCh; ++k) sg[k] = sgx[k] = 0.f;
+  auto push = [&](const Vec16* pd, const Vec16* px, uint32_t bits) {
+    float d[kCh], f[kCh];
+    hold_load<U>(pd, d);
+    hold_load<U>(px, f);
+    mask_grad<kRelu>(d, bits);
+#pragma unroll
+    for (int k = 0; k < kCh; ++k) {
+      sg[k] += d[k];
+      sgx[k] = fmaf(d[k], f[k] - mu[k], sgx[k]);
+    }
+  };
   if (u < units) {
 #pragma unroll
     for (int k = 0; k < kCh; ++k) mu[k] = mean[u * kCh + k];
-    for (int j = lane; j < nh; j += RL) {
-      const size_t i = (r0 + j) * units + u;
-      hold_copy<U>(hdy + (j * CB + col) * V, dy, i);
-      hold_copy<U>(hx + (j * CB + col) * V, x, i);
-      if constexpr (kRelu) hm[j * CB + col] = mask[i];
+    for (int k = 0; k < hn; ++k) {
+      const size_t i = i_h + k * ustep;
+      hold_copy<U>(hdy + (size_t)k * SV, dy, i);
+      hold_copy<U>(hx + (size_t)k * SV, x, i);
+      if constexpr (kRelu) mask_copy(hm + (size_t)k * kT, mask, i, nm);
     }
-    size_t r = r0 + nh + lane;
-    for (; r + 3 * RL < r1; r += 4 * RL) {
-      float d[4][kCh], f[4][kCh];
-      uint32_t bits[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const size_t i = (r + j * RL) * units + u;
-        Unit<U>::load(dy, i, d[j]);
-        Unit<U>::load(x, i, f[j]);
-        if constexpr (kRelu) bits[j] = mask[i];
-      }
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        mask_grad<kRelu>(d[j], bits[j]);
-#pragma unroll
-        for (int k = 0; k < kCh; ++k) {
-          sg[k] += d[j][k];
-          sgx[k] = fmaf(d[j][k], f[j][k] - mu[k], sgx[k]);
-        }
-      }
-    }
-    for (; r < r1; r += RL) {
-      const size_t i = r * units + u;
-      float d[kCh], f[kCh];
-      Unit<U>::load(dy, i, d);
-      Unit<U>::load(x, i, f);
-      if constexpr (kRelu) mask_grad<kRelu>(d, mask[i]);
-#pragma unroll
-      for (int k = 0; k < kCh; ++k) {
-        sg[k] += d[k];
-        sgx[k] = fmaf(d[k], f[k] - mu[k], sgx[k]);
-      }
-    }
-    cp_async_wait_all();
-    for (int j = lane; j < nh; j += RL) {
-      float d[kCh], f[kCh];
-      hold_load<U>(hdy + (j * CB + col) * V, d);
-      hold_load<U>(hx + (j * CB + col) * V, f);
-      if constexpr (kRelu) mask_grad<kRelu>(d, hm[j * CB + col]);
-#pragma unroll
-      for (int k = 0; k < kCh; ++k) {
-        sg[k] += d[k];
-        sgx[k] = fmaf(d[k], f[k] - mu[k], sgx[k]);
-      }
-    }
+    cp_async_commit();
+    auto issue = [&](int k, int slot) { issue_at(slot, i_s + k * ustep); };
+    ring_fill<kBwdStages>(sn, issue);
+    cp_async_wait<kBwdStages>();
+    for (int k = 0; k < hn; ++k)
+      push(hdy + (size_t)k * SV, hx + (size_t)k * SV,
+           kRelu ? mask_byte(hm[(size_t)k * kT], mask, i_h + k * ustep) : 0u);
+    ring_drain<kBwdStages>(sn, issue, [&](int k, int slot) {
+      push(slot_dy(slot), slot_x(slot), kRelu ? mask_byte(*slot_m(slot), mask, i_s + k * ustep) : 0u);
+    });
   }
   tree_sum2<kCh>(sg, sgx, lane, CB, RL);
   const int G = gridDim.x;
@@ -753,27 +837,23 @@ __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_bwd_fused_kernel(
     D[k] = s_D[col * kCh + k];
     E[k] = s_E[col * kCh + k];
   }
-  const int ns = rows - nh;
-  for (int k = lane < ns ? (ns - 1 - lane) / RL : -1; k >= 0; k -= 2) {
-    const size_t i0 = (r0 + nh + lane + (size_t)k * RL) * units + u, i1 = i0 - (size_t)RL * units;
-    float d0[kCh], d1[kCh], f0[kCh], f1[kCh];
-    uint32_t b0 = 0, b1 = 0;
-    Unit<U>::load(dy, i0, d0);
-    Unit<U>::load(x, i0, f0);
-    if constexpr (kRelu) b0 = __ldcs(mask + i0);
-    if (k >= 1) {
-      Unit<U>::load(dy, i1, d1);
-      Unit<U>::load(x, i1, f1);
-      if constexpr (kRelu) b1 = __ldcs(mask + i1);
-    }
-    bwd_row<U, kRelu, kRes>(i0, mu, A, D, E, dx, dres, d0, f0, b0);
-    if (k >= 1) bwd_row<U, kRelu, kRes>(i1, mu, A, D, E, dx, dres, d1, f1, b1);
-  }
-  for (int j = lane; j < nh; j += RL) {
+  // phase 2: streamed rows through the ring, last read first, then the held rows
+  auto unit2 = [&](int k) { return i_s + (size_t)(sn - 1 - k) * ustep; };
+  auto issue2 = [&](int k, int slot) { issue_at(slot, unit2(k)); };
+  ring_fill<kBwdStages>(sn, issue2);
+  ring_drain<kBwdStages>(sn, issue2, [&](int k, int slot) {
+    const size_t i = unit2(k);
     float d[kCh], f[kCh];
-    hold_load<U>(hdy + (j * CB + col) * V, d);
-    hold_load<U>(hx + (j * CB + col) * V, f);
-    bwd_row<U, kRelu, kRes>((r0 + j) * units + u, mu, A, D, E, dx, dres, d, f, kRelu ? hm[j * CB + col] : 0u);
+    hold_load<U>(slot_dy(slot), d);
+    hold_load<U>(slot_x(slot), f);
+    bwd_row<U, kRelu, kRes>(i, mu, A, D, E, dx, dres, d, f, kRelu ? mask_byte(*slot_m(slot), mask, i) : 0u);
+  });
+  for (int k = 0; k < hn; ++k) {
+    const size_t i = i_h + k * ustep;
+    float d[kCh], f[kCh];
+    hold_load<U>(hdy + (size_t)k * SV, d);
+    hold_load<U>(hx + (size_t)k * SV, f);
+    bwd_row<U, kRelu, kRes>(i, mu, A, D, E, dx, dres, d, f, kRelu ? mask_byte(hm[(size_t)k * kT], mask, i) : 0u);
   }
 }
 
@@ -968,15 +1048,19 @@ struct FusedPlan {
   size_t rpc;   // rows per chunk, a multiple of RL
   int G;        // chunks (gridDim.x)
   int held;     // rows of a chunk held in shared memory: a multiple of RL, or rpc
-  size_t smem;  // dynamic shared memory per block
+  int depth;    // ring row-steps: 0 when the whole chunk is held
+  size_t held_bytes, smem;   // shared memory of the held rows; all dynamic shared memory per block
 };
 
-// Bytes of shared memory per held block row.
-size_t held_row_bytes(int bwd, int dtype, const Geo& g) {
+// Bytes of shared memory per held block row: one unit per thread of dy and x (backward) or x, plus a 4-byte mask
+// word (backward).  A ring stage holds the same for the kT threads of a row-step.
+size_t unit_bytes(int bwd, int dtype) {
   const size_t vec = (size_t)kCh * (dtype == WIRE_F32 ? 4 : 2);
-  return ((size_t)1 << g.shift) * (bwd ? 2 * vec + 1 : vec);
+  return bwd ? 2 * vec + 4 : vec;
 }
 
+// The whole chunk is held when it fits; otherwise the ring of kFwdStages / kBwdStages row-steps comes first and the
+// held rows get what is left (at most `cap` bytes of them when cap >= 0).
 bool fused_plan(int bwd, int dtype, size_t M, int C, long long cap, FusedPlan* p) {
   const int dt = dtype_index(dtype);
   const FusedDev* d = fused_dev();
@@ -987,13 +1071,33 @@ bool fused_plan(int bwd, int dtype, size_t M, int C, long long cap, FusedPlan* p
   const size_t want = (size_t)(blocks / g.ncb), rl = (size_t)g.rl;
   size_t rpc = (M + want - 1) / want;
   rpc = (rpc < rl ? rl : (rpc + rl - 1) / rl * rl);
-  size_t budget = d->dyn[bwd ? 1 : 0][dt];
-  if (cap >= 0 && (size_t)cap < budget) budget = (size_t)cap;
-  const size_t row = held_row_bytes(bwd, dtype, g);
-  size_t held = budget / row;
-  held = held >= rpc ? rpc : held / rl * rl;
-  *p = FusedPlan{g, rpc, (int)((M + rpc - 1) / rpc), (int)held, (held * row + 15) & ~(size_t)15};
+  const size_t dyn = d->dyn[bwd ? 1 : 0][dt], capb = cap >= 0 ? (size_t)cap : dyn;
+  const size_t row = ((size_t)1 << g.shift) * unit_bytes(bwd, dtype);
+  size_t held = rpc;
+  int depth = 0;
+  if (rpc * row > (dyn < capb ? dyn : capb)) {
+    depth = bwd ? kBwdStages : kFwdStages;
+    const size_t ring = (size_t)depth * kT * unit_bytes(bwd, dtype);
+    if (ring > dyn) return false;
+    const size_t budget = dyn - ring < capb ? dyn - ring : capb;
+    held = budget / row / rl * rl;
+  }
+  const size_t hb = held * row;
+  *p = FusedPlan{g, rpc, (int)((M + rpc - 1) / rpc), (int)held, depth, hb,
+                 hb + (size_t)depth * kT * unit_bytes(bwd, dtype)};
   return true;
+}
+
+// Bytes a launch moves between HBM (or L2) and the SMs: every row once, and the rows a block does not hold again in
+// phase 2 (dy, x and the mask backward; x forward), plus the residual read, the outputs and the mask written.
+size_t fused_bytes(const FusedPlan& p, int bwd, int dtype, size_t M, int C, bool relu, bool res) {
+  const size_t last = M - (size_t)(p.G - 1) * p.rpc;
+  const size_t held = (size_t)(p.G - 1) * ((size_t)p.held < p.rpc ? p.held : p.rpc) +
+                      ((size_t)p.held < last ? p.held : last);
+  const size_t e = (size_t)C * (dtype == WIRE_F32 ? 4 : 2), m = relu ? (size_t)C / kCh : 0;   // per row
+  const size_t reread = (M - held) * (bwd ? 2 * e + m : e);
+  if (bwd) return M * (3 * e + m) + (res ? M * e : 0) + reread;
+  return M * (2 * e + m) + (res ? M * e : 0) + reread;
 }
 
 template <class... P, class... A>
@@ -1094,10 +1198,12 @@ cudaError_t launch_bn_act_fwd_stats_local(const void* x, int dtype, size_t M, in
   return cudaGetLastError();
 }
 
-bool bn_act_fused_plan(int bwd, int dtype, size_t M, int C, long long cap, BnFusedPlan* out) {
+bool bn_act_fused_plan(int bwd, int dtype, size_t M, int C, long long cap, int relu, int residual,
+                       BnFusedPlan* out) {
   FusedPlan p;
   if (!fused_plan(bwd, dtype, M, C, cap, &p)) return false;
-  *out = BnFusedPlan{2 * (size_t)p.G * (size_t)C, p.g.ncb, p.rpc, p.held, p.smem, fused_dev()->sms * kResBlocksPerSM};
+  *out = BnFusedPlan{2 * (size_t)p.G * (size_t)C, p.g.ncb, p.rpc, p.held, p.held_bytes, p.depth, p.smem,
+                     fused_bytes(p, bwd, dtype, M, C, relu != 0, residual != 0), fused_dev()->sms * kResBlocksPerSM};
   return true;
 }
 

@@ -49,20 +49,26 @@ cudaError_t launch_bn_act_bwd_apply(const void* dy, const void* x, const uint8_t
 //   bwd   bwd_reduce then bwd_apply (dividing by M) in one launch: same outputs, dweight and dbias
 //
 // Each is one cooperative launch of exactly one wave; a grid barrier separates the reduction from the apply.  A block
-// holds as many rows of its chunk as fit in its share of shared memory (at most `cap` bytes when cap >= 0; cap = 0
-// streams every row twice), so the apply reads most of its input from on chip or L2 instead of HBM.  bn_act_fused_plan
-// tells whether the pass can run at (M, C, dtype) on the current device (false: use the two-pass kernels; the
-// launchers then return cudaErrorNotSupported) and fills in its workspace: ws_floats floats and `counters` zeroed
-// uint32 counters, per launch as for the two-pass kernels, except that the counters are left non-zero.
+// holds its whole chunk in its share of shared memory when it fits; otherwise a ring of a few row-steps streams the
+// rest of the chunk through shared memory with asynchronous copies, and the held rows get the space the ring leaves
+// (at most `cap` bytes of them when cap >= 0; cap = 0 streams every row twice), so the apply reads most of its input
+// from on chip or L2 instead of HBM.  Results do not depend on how many rows are held.  bn_act_fused_plan tells
+// whether the pass can run at (M, C, dtype) on the current device (false: use the two-pass kernels; the launchers
+// then return cudaErrorNotSupported) and fills in its workspace: ws_floats floats and `counters` zeroed uint32
+// counters, per launch as for the two-pass kernels, except that the counters are left non-zero.
 struct BnFusedPlan {
   size_t ws_floats;
   int counters;
   size_t rows_per_chunk;   // rows of a block's chunk (the last chunk may have fewer)
   int held_rows;           // rows of a chunk held in shared memory from the reduction to the apply
-  size_t held_bytes;       // dynamic shared memory per block
+  size_t held_bytes;       // shared memory of the held rows per block
+  int ring_depth;          // row-steps of the streaming ring (0: the whole chunk is held)
+  size_t smem_bytes;       // dynamic shared memory per block: held rows and ring
+  size_t bytes_moved;      // bytes a launch with (relu, residual) reads and writes, re-reads of streamed rows included
   int wave_blocks;         // blocks in one wave on this device: the grid is at most this large
 };
-bool bn_act_fused_plan(int bwd, int dtype, size_t M, int C, long long cap, BnFusedPlan* plan);
+bool bn_act_fused_plan(int bwd, int dtype, size_t M, int C, long long cap, int relu, int residual,
+                       BnFusedPlan* plan);
 cudaError_t launch_bn_act_fwd(const void* x, const void* residual, int dtype, size_t M, int C, float eps,
                               float momentum, float* running_mean, float* running_var, float* save_mean,
                               float* save_invstd, const float* weight, const float* bias, int relu, void* y,
