@@ -245,4 +245,5 @@ PYBIND11_MODULE(_cuda, m) {
   bind_cuda_ring(m);
   bind_cuda_compress(m);
   bind_cuda_bn(m);
+  bind_cuda_ln(m);
 }

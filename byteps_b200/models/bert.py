@@ -8,6 +8,8 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from ..ops.ln import DropoutAddLayerNorm
+
 
 @dataclass
 class BertConfig:
@@ -20,6 +22,9 @@ class BertConfig:
     type_vocab_size: int = 2
     dropout: float = 0.1
     layer_norm_eps: float = 1e-12
+    # norm1 / norm2 of every layer as DropoutAddLayerNorm: the dropout, residual add and LayerNorm of each junction
+    # run as one fused kernel per direction on CUDA (same parameters and state_dict as the stock layers)
+    fused_norm: bool = False
 
 
 class BertEmbeddings(nn.Module):
@@ -36,23 +41,33 @@ class BertEmbeddings(nn.Module):
         return self.drop(self.norm(self.word(ids) + self.pos(pos) + self.token_type(type_ids)))
 
 
+def _junction_norm(c: BertConfig) -> nn.LayerNorm:
+    if c.fused_norm:
+        return DropoutAddLayerNorm(c.hidden_size, eps=c.layer_norm_eps, p=c.dropout)
+    return nn.LayerNorm(c.hidden_size, eps=c.layer_norm_eps)
+
+
 class BertLayer(nn.Module):
     def __init__(self, c: BertConfig):
         super().__init__()
         self.h, self.d = c.num_heads, c.hidden_size // c.num_heads
         self.qkv = nn.Linear(c.hidden_size, 3 * c.hidden_size)
         self.proj = nn.Linear(c.hidden_size, c.hidden_size)
-        self.norm1 = nn.LayerNorm(c.hidden_size, eps=c.layer_norm_eps)
+        self.norm1 = _junction_norm(c)
         self.fc1 = nn.Linear(c.hidden_size, c.intermediate_size)
         self.fc2 = nn.Linear(c.intermediate_size, c.hidden_size)
-        self.norm2 = nn.LayerNorm(c.hidden_size, eps=c.layer_norm_eps)
+        self.norm2 = _junction_norm(c)
         self.p = c.dropout
+        self.fused_norm = c.fused_norm
 
     def forward(self, x, mask=None):
         b, s, e = x.shape
         q, k, v = self.qkv(x).view(b, s, 3, self.h, self.d).permute(2, 0, 3, 1, 4)
         a = F.scaled_dot_product_attention(q, k, v, attn_mask=mask, dropout_p=self.p if self.training else 0.0)
         a = a.transpose(1, 2).reshape(b, s, e)
+        if self.fused_norm:
+            x = self.norm1(self.proj(a), x)
+            return self.norm2(self.fc2(F.gelu(self.fc1(x))), x)
         x = self.norm1(x + F.dropout(self.proj(a), self.p, self.training))
         y = self.fc2(F.gelu(self.fc1(x)))
         return self.norm2(x + F.dropout(y, self.p, self.training))

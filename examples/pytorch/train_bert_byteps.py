@@ -20,13 +20,15 @@ p.add_argument("--seq-len", type=int, default=128)
 p.add_argument("--steps", type=int, default=20)
 p.add_argument("--warmup-steps", type=int, default=5)
 p.add_argument("--no-cuda", action="store_true", help="CPU run over gloo (unfused optimizer, fp32)")
+p.add_argument("--fused-norm", action="store_true",
+               help="fused dropout + residual add + LayerNorm kernels at the encoder layers' junctions")
 args = p.parse_args()
 bps.init()
 cuda = torch.cuda.is_available() and not args.no_cuda
 if cuda:
     torch.cuda.set_device(bps.local_rank())
 dev = torch.device("cuda", bps.local_rank()) if cuda else torch.device("cpu")
-model = get_model(args.model).to(dev)
+model = get_model(args.model, fused_norm=args.fused_norm).to(dev)
 if cuda:
     model = model.to(torch.bfloat16)
 opt = bps.DistributedOptimizer(torch.optim.AdamW(model.parameters(), lr=1e-4, weight_decay=0.01),
