@@ -246,4 +246,5 @@ PYBIND11_MODULE(_cuda, m) {
   bind_cuda_compress(m);
   bind_cuda_bn(m);
   bind_cuda_ln(m);
+  bind_cuda_xent(m);
 }

@@ -9,6 +9,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from ..ops.ln import DropoutAddLayerNorm
+from ..ops.xent import softmax_cross_entropy
 
 
 @dataclass
@@ -25,6 +26,9 @@ class BertConfig:
     # norm1 / norm2 of every layer as DropoutAddLayerNorm: the dropout, residual add and LayerNorm of each junction
     # run as one fused kernel per direction on CUDA (same parameters and state_dict as the stock layers)
     fused_norm: bool = False
+    # the MLM loss through ops.xent.softmax_cross_entropy: one fused kernel per direction on CUDA reads the
+    # low-precision logits in place of the fp32 cast and log-softmax of F.cross_entropy (same value)
+    fused_loss: bool = False
 
 
 class BertEmbeddings(nn.Module):
@@ -105,7 +109,10 @@ class BertForPreTraining(nn.Module):
         nsp_logits = self.nsp(pooled)
         if mlm_labels is None:
             return logits, nsp_logits
-        loss = F.cross_entropy(logits.view(-1, logits.shape[-1]).float(), mlm_labels.view(-1), ignore_index=-100)
+        if self.config.fused_loss:
+            loss = softmax_cross_entropy(logits.view(-1, logits.shape[-1]), mlm_labels.view(-1), ignore_index=-100)
+        else:
+            loss = F.cross_entropy(logits.view(-1, logits.shape[-1]).float(), mlm_labels.view(-1), ignore_index=-100)
         if nsp_labels is not None:
             loss = loss + F.cross_entropy(nsp_logits.float(), nsp_labels)
         return loss

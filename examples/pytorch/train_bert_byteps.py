@@ -22,13 +22,15 @@ p.add_argument("--warmup-steps", type=int, default=5)
 p.add_argument("--no-cuda", action="store_true", help="CPU run over gloo (unfused optimizer, fp32)")
 p.add_argument("--fused-norm", action="store_true",
                help="fused dropout + residual add + LayerNorm kernels at the encoder layers' junctions")
+p.add_argument("--fused-loss", action="store_true",
+               help="fused softmax cross-entropy kernels for the masked-LM loss")
 args = p.parse_args()
 bps.init()
 cuda = torch.cuda.is_available() and not args.no_cuda
 if cuda:
     torch.cuda.set_device(bps.local_rank())
 dev = torch.device("cuda", bps.local_rank()) if cuda else torch.device("cpu")
-model = get_model(args.model, fused_norm=args.fused_norm).to(dev)
+model = get_model(args.model, fused_norm=args.fused_norm, fused_loss=args.fused_loss).to(dev)
 if cuda:
     model = model.to(torch.bfloat16)
 opt = bps.DistributedOptimizer(torch.optim.AdamW(model.parameters(), lr=1e-4, weight_decay=0.01),
