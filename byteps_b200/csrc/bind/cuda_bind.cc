@@ -247,4 +247,5 @@ PYBIND11_MODULE(_cuda, m) {
   bind_cuda_bn(m);
   bind_cuda_ln(m);
   bind_cuda_xent(m);
+  bind_cuda_fp8(m);
 }

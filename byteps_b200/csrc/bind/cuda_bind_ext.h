@@ -9,3 +9,4 @@ void bind_cuda_compress(pybind11::module_& m);
 void bind_cuda_bn(pybind11::module_& m);
 void bind_cuda_ln(pybind11::module_& m);
 void bind_cuda_xent(pybind11::module_& m);
+void bind_cuda_fp8(pybind11::module_& m);

@@ -8,6 +8,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from ..ops.fp8 import Fp8Linear
 from ..ops.ln import DropoutAddLayerNorm
 from ..ops.xent import softmax_cross_entropy
 
@@ -29,6 +30,9 @@ class BertConfig:
     # the MLM loss through ops.xent.softmax_cross_entropy: one fused kernel per direction on CUDA reads the
     # low-precision logits in place of the fp32 cast and log-softmax of F.cross_entropy (same value)
     fused_loss: bool = False
+    # qkv, proj, fc1 and fc2 of every encoder layer as ops.fp8.Fp8Linear: FP8 GEMMs with delayed scaling on sm_90
+    # (same parameters and state_dict as nn.Linear); the heads stay in the model's dtype
+    fp8_linear: bool = False
 
 
 class BertEmbeddings(nn.Module):
@@ -51,15 +55,19 @@ def _junction_norm(c: BertConfig) -> nn.LayerNorm:
     return nn.LayerNorm(c.hidden_size, eps=c.layer_norm_eps)
 
 
+def _encoder_linear(c: BertConfig, i: int, o: int) -> nn.Linear:
+    return Fp8Linear(i, o) if c.fp8_linear else nn.Linear(i, o)
+
+
 class BertLayer(nn.Module):
     def __init__(self, c: BertConfig):
         super().__init__()
         self.h, self.d = c.num_heads, c.hidden_size // c.num_heads
-        self.qkv = nn.Linear(c.hidden_size, 3 * c.hidden_size)
-        self.proj = nn.Linear(c.hidden_size, c.hidden_size)
+        self.qkv = _encoder_linear(c, c.hidden_size, 3 * c.hidden_size)
+        self.proj = _encoder_linear(c, c.hidden_size, c.hidden_size)
         self.norm1 = _junction_norm(c)
-        self.fc1 = nn.Linear(c.hidden_size, c.intermediate_size)
-        self.fc2 = nn.Linear(c.intermediate_size, c.hidden_size)
+        self.fc1 = _encoder_linear(c, c.hidden_size, c.intermediate_size)
+        self.fc2 = _encoder_linear(c, c.intermediate_size, c.hidden_size)
         self.norm2 = _junction_norm(c)
         self.p = c.dropout
         self.fused_norm = c.fused_norm

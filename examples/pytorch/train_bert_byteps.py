@@ -24,13 +24,16 @@ p.add_argument("--fused-norm", action="store_true",
                help="fused dropout + residual add + LayerNorm kernels at the encoder layers' junctions")
 p.add_argument("--fused-loss", action="store_true",
                help="fused softmax cross-entropy kernels for the masked-LM loss")
+p.add_argument("--fp8-linear", action="store_true",
+               help="FP8 GEMMs with delayed scaling for the encoder layers' linear layers (sm_90)")
 args = p.parse_args()
 bps.init()
 cuda = torch.cuda.is_available() and not args.no_cuda
 if cuda:
     torch.cuda.set_device(bps.local_rank())
 dev = torch.device("cuda", bps.local_rank()) if cuda else torch.device("cpu")
-model = get_model(args.model, fused_norm=args.fused_norm, fused_loss=args.fused_loss).to(dev)
+model = get_model(args.model, fused_norm=args.fused_norm, fused_loss=args.fused_loss,
+                  fp8_linear=args.fp8_linear).to(dev)
 if cuda:
     model = model.to(torch.bfloat16)
 opt = bps.DistributedOptimizer(torch.optim.AdamW(model.parameters(), lr=1e-4, weight_decay=0.01),
