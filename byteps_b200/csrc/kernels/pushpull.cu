@@ -68,14 +68,16 @@ __global__ void __launch_bounds__(512) pushpull_packed_kernel(PeerView pv, const
   barrier_peers(pv, channel);
   EpiScale epi{scale};
   if (one_shot) {
-    // every rank reduces every unit (fixed peer order -> bit-identical results
-    // on all ranks) and scatters straight into the user tensors.
+    // every rank reduces every unit and scatters straight into the user tensors.
+    // Shard r is summed in the peer order its owner uses in two-shot mode (rotation r + 1),
+    // so the results are bit-identical on all ranks and in both modes.
     SegCursor cur;
     bool inited = false;
     for (int r = 0; r < pv.world; ++r) {
       size_t s0, s1;
       shard_units_of<E>(total_groups, pv.world, r, &s0, &s1);
-      reduce_phase<W, kUnroll>(pv, stage_off, s0, s1, nvls != 0, 0, epi, [&](const float* f, size_t unit) {
+      const int rot = r + 1 == pv.world ? 0 : r + 1;
+      reduce_phase<W, kUnroll>(pv, stage_off, s0, s1, nvls != 0, rot, epi, [&](const float* f, size_t unit) {
         int64_t e = (int64_t)unit * E;
         if (!inited) {
           cur.init(segs, nsegs, e);

@@ -60,7 +60,10 @@ struct LaunchCfg {
 };
 
 // ---- in-place exchange on the symmetric arena ---------------------------------
-// data at [off, off + n*elem) of every rank's arena is replaced by scale * sum.
+// data at [off, off + n*elem) of every rank's arena is replaced by scale * sum.  The kernels work in
+// groups of 8 elements: when n is not a multiple of 8, the elements up to the next multiple of 8
+// ([off + n*elem, off + pad8(n)*elem)) are exchanged too and must be free to change.  The same holds
+// for launch_pushpull_inplace_tma, launch_reduce_scatter and launch_all_gather.
 cudaError_t launch_pushpull_inplace(const PeerView& pv, int wire, size_t off_bytes, size_t nelem, float scale,
                                     const LaunchCfg& cfg, cudaStream_t stream);
 
