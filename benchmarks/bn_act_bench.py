@@ -16,7 +16,11 @@ are the least each fused pass must move, computed from the shape (e = element by
     single:bwd  read dy, x [, mask] once; write dx [, dres]  N e (3 [+1]) [+ N / 8]   (bwd_reduce + bwd_apply)
 
 The fused:fwd / fused:bwd rows sum the two-pass kernels; the single rows are the single-launch kernels the module
-takes where their plan allows it.  Those rows also print the bytes the launch actually moves (the plan's
+takes where their plan allows it.  On the expanded shapes the junction rows time bn3's backward at a ResNet block
+junction, where the output has two consumers: junction:add+bwd is torch's add of the two gradients followed by the
+single-launch backward (what autograd did before the kernel took both), junction:bwd2 the single-launch backward
+reading both gradients.  Their bytes are what the launches move (the add: 3 N e; the plans' bytes_moved), and the
+table ends with the saving per ResNet-50 step over its 15 junctions.  Those rows also print the bytes the launch actually moves (the plan's
 bytes_moved: the rows a block does not hold are read twice) with the share of peak over them, and the plan's held
 rows per chunk and ring depth.  Every timed launch moves to the next of enough copies of the tensors that the
 launches of a row touch more than --rotate-mb together, so no pass finds its input in the 50 MB L2 from the launch
@@ -40,6 +44,8 @@ PEAK_GBS = 3350.0
 SHAPES = [(64, 112, 112), (64, 56, 56), (256, 56, 56), (128, 56, 56), (128, 28, 28), (512, 28, 28),
           (256, 28, 28), (256, 14, 14), (1024, 14, 14), (512, 14, 14), (512, 7, 7), (2048, 7, 7)]
 EXPANDED = {(256, 56, 56), (512, 28, 28), (1024, 14, 14), (2048, 7, 7)}
+# ResNet-50's block junctions per expanded shape: identity and downsample skip paths of the block that follows
+JUNCTIONS = {(256, 56, 56): 3, (512, 28, 28): 4, (1024, 14, 14): 6, (2048, 7, 7): 2}
 
 
 def gpu_info():
@@ -97,7 +103,7 @@ def main():
             relu, res = var != "none", var == "relu_res"
             g = torch.Generator(device=dev).manual_seed(0)
             mb = n // 8 if relu else 0
-            k = max(1, int(-(-args.rotate_mb * 1e6 // (n * e * (5 if res else 3) + 2 * mb))))
+            k = max(1, int(-(-args.rotate_mb * 1e6 // (n * e * (7 if res else 3) + 2 * mb))))
 
             def copies():
                 x = torch.randn(args.batch, c, h, w, device=dev, generator=g).to(dt).contiguous(
@@ -105,8 +111,10 @@ def main():
                 return dict(x=x, r=torch.randn_like(x) if res else None, dy=torch.randn_like(x),
                             y=torch.empty_like(x), dx=torch.empty_like(x),
                             dres=torch.empty_like(x) if res else None,
+                            dy2=torch.randn_like(x) if res else None, dsum=torch.empty_like(x) if res else None,
                             mask=torch.empty(m, c // 8, dtype=torch.uint8, device=dev) if relu else None)
 
+            first = len(rows)
             T = [copies() for _ in range(k)]
             P = [{key: (0 if t is None else t.data_ptr()) for key, t in tk.items()} for tk in T]
             wt, bs = torch.ones(c, device=dev), torch.zeros(c, device=dev)
@@ -172,6 +180,29 @@ def main():
                                      us=ms * 1e3, held_rows=plan["held_rows"], rows_per_chunk=plan["rows_per_chunk"],
                                      ring_depth=plan["ring_depth"], bytes_moved=plan["bytes_moved"]))
 
+                if res:
+                    jplan = cu.bn_act_plan(1, code, m, c, relu=relu, residual=True, dy2=True)
+
+                    def bwd(i, dy, dy2=0):
+                        cu.bn_act_bwd(dy, P[i]["x"], P[i]["mask"], code, m, c, mean.data_ptr(), inv.data_ptr(),
+                                      wt.data_ptr(), dw.data_ptr(), db.data_ptr(), P[i]["dx"], P[i]["dres"],
+                                      ws1.data_ptr(), zeroed(), s, -1, dy2)
+
+                    def add_bwd(i):
+                        torch.add(T[i]["dy"], T[i]["dy2"], out=T[i]["dsum"])
+                        bwd(i, P[i]["dsum"])
+
+                    for name, plan, fn in (("add+bwd", bplan, add_bwd),
+                                           ("bwd2", jplan, lambda i: bwd(i, P[i]["dy"], P[i]["dy2"]))):
+                        launch[0] = 0
+                        ctrs.zero_()
+                        ms = timed(fn, k)
+                        moved = plan["bytes_moved"] + (3 * n * e if name == "add+bwd" else 0)
+                        rows.append(dict(shape=[c, h, w], variant=var, impl="junction", kind=name, bytes=moved,
+                                         us=ms * 1e3, held_rows=plan["held_rows"],
+                                         rows_per_chunk=plan["rows_per_chunk"], ring_depth=plan["ring_depth"],
+                                         bytes_moved=moved))
+
             # stock sequence on the same tensors
             XS = [t["x"].detach().requires_grad_(True) for t in T]
             RS = [t["r"].detach().requires_grad_(True) if res else None for t in T]
@@ -197,11 +228,11 @@ def main():
             for side in ("fwd", "bwd"):
                 rows.append(dict(shape=[c, h, w], variant=var, impl="fused", kind=side, bytes=tot[side][1],
                                  us=tot[side][0] * 1e3))
-            for row in rows[-(len(passes) + len(single) + 4):]:
+            for row in rows[first:]:
                 gbs = row["bytes"] / (row["us"] * 1e3)
                 row["gbs"], row["peak_share"] = gbs, gbs / PEAK_GBS
                 extra = ""
-                if row["impl"] == "single":
+                if row["impl"] in ("single", "junction"):
                     row["moved_share"] = row["bytes_moved"] / (row["us"] * 1e3) / PEAK_GBS
                     extra = " %9.1f %6.0f%%  held %d/%d ring %d" % (
                         row["bytes_moved"] / 1e6, 100 * row["moved_share"], row["held_rows"], row["rows_per_chunk"],
@@ -214,6 +245,12 @@ def main():
     g_tot = sum(r_["us"] for r_ in rows if r_["impl"] == "single")
     s_tot = sum(r_["us"] for r_ in rows if r_["impl"] == "stock")
     print("sum over the variants above: two-pass %.0f us, single-launch %.0f us, stock %.0f us" % (f_tot, g_tot, s_tot))
+    junction = {(tuple(r_["shape"]), r_["kind"]): r_["us"] for r_ in rows if r_["impl"] == "junction"}
+    if junction:
+        saved = sum(cnt * (junction[(shp, "add+bwd")] - junction[(shp, "bwd2")]) for shp, cnt in JUNCTIONS.items()
+                    if (shp, "bwd2") in junction)
+        print("ResNet-50 junctions (%s): add+bwd -> bwd2 saves %.0f us per step" % (
+            ", ".join("%dx%dx%d: %d" % (shp + (cnt,)) for shp, cnt in JUNCTIONS.items()), saved))
     if args.json:
         with open(args.json, "w") as fh:
             json.dump({"gpu": info, "batch": args.batch, "rows": rows}, fh, indent=1)

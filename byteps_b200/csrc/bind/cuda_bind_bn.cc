@@ -60,9 +60,10 @@ void bind_cuda_bn(py::module_& m) {
      "total: device float holding the row count to divide by (bn_sync_stats writes it); 0 divides by M");
 
   // ---- single-launch passes
-  m.def("bn_act_plan", [](int bwd, int dtype, size_t M, int C, long long cap, bool relu, bool residual) -> py::object {
+  m.def("bn_act_plan", [](int bwd, int dtype, size_t M, int C, long long cap, bool relu, bool residual,
+                          bool dy2) -> py::object {
     BnFusedPlan p;
-    if (!bn_act_fused_plan(bwd, dtype, M, C, cap, relu ? 1 : 0, residual ? 1 : 0, &p)) return py::none();
+    if (!bn_act_fused_plan(bwd, dtype, M, C, cap, relu ? 1 : 0, residual ? 1 : 0, dy2 ? 1 : 0, &p)) return py::none();
     py::dict d;
     d["ws_floats"] = p.ws_floats;
     d["counters"] = p.counters;
@@ -75,10 +76,11 @@ void bind_cuda_bn(py::module_& m) {
     d["wave_blocks"] = p.wave_blocks;
     return d;
   }, py::arg("bwd"), py::arg("dtype"), py::arg("M"), py::arg("C"), py::arg("cap") = -1, py::arg("relu") = false,
-     py::arg("residual") = false,
+     py::arg("residual") = false, py::arg("dy2") = false,
      "plan of the single-launch bn_act_fwd (bwd=0) / bn_act_bwd (bwd=1) at (M, C, dtype) on the current device, or "
-     "None when it cannot run there; cap >= 0 limits the bytes of rows a block holds in shared memory.  relu and "
-     "residual only select the variant whose bytes_moved is reported");
+     "None when it cannot run there; cap >= 0 limits the bytes of rows a block holds in shared memory.  residual "
+     "selects the backward's shared-memory layout; relu, residual and dy2 (a second gradient, backward with a "
+     "residual) select the variant whose bytes_moved is reported");
   m.def("bn_act_fwd", [](uintptr_t x, uintptr_t residual, int dtype, size_t M, int C, float eps, float momentum,
                          uintptr_t running_mean, uintptr_t running_var, uintptr_t save_mean, uintptr_t save_invstd,
                          uintptr_t weight, uintptr_t bias, bool relu, uintptr_t y, uintptr_t mask, uintptr_t ws,
@@ -94,14 +96,18 @@ void bind_cuda_bn(py::module_& m) {
      py::arg("ws"), py::arg("counters"), py::arg("stream"), py::arg("cap") = -1);
   m.def("bn_act_bwd", [](uintptr_t dy, uintptr_t x, uintptr_t mask, int dtype, size_t M, int C, uintptr_t mean,
                          uintptr_t invstd, uintptr_t weight, uintptr_t dweight, uintptr_t dbias, uintptr_t dx,
-                         uintptr_t dresidual, uintptr_t ws, uintptr_t counters, uintptr_t s, long long cap) {
-    chk(launch_bn_act_bwd((const void*)dy, (const void*)x, (const uint8_t*)mask, dtype, M, C, (const float*)mean,
-                          (const float*)invstd, (const float*)weight, (float*)dweight, (float*)dbias, (void*)dx,
-                          (void*)dresidual, (float*)ws, (uint32_t*)counters, cap, (cudaStream_t)s),
+                         uintptr_t dresidual, uintptr_t ws, uintptr_t counters, uintptr_t s, long long cap,
+                         uintptr_t dy2) {
+    chk(launch_bn_act_bwd((const void*)dy, (const void*)dy2, (const void*)x, (const uint8_t*)mask, dtype, M, C,
+                          (const float*)mean, (const float*)invstd, (const float*)weight, (float*)dweight,
+                          (float*)dbias, (void*)dx, (void*)dresidual, (float*)ws, (uint32_t*)counters, cap,
+                          (cudaStream_t)s),
         "bn_act_bwd");
   }, py::arg("dy"), py::arg("x"), py::arg("mask"), py::arg("dtype"), py::arg("M"), py::arg("C"), py::arg("mean"),
      py::arg("invstd"), py::arg("weight"), py::arg("dweight"), py::arg("dbias"), py::arg("dx"), py::arg("dresidual"),
-     py::arg("ws"), py::arg("counters"), py::arg("stream"), py::arg("cap") = -1);
+     py::arg("ws"), py::arg("counters"), py::arg("stream"), py::arg("cap") = -1, py::arg("dy2") = 0,
+     "dy2: 0, or a second gradient of the output laid out as dy (M x C, 16-byte aligned; needs dresidual), summed "
+     "with dy inside the kernel");
 
   // ---- synchronised batch norm
   m.def("bn_act_load_kernels", []() { chk(bn_act_load_kernels(), "bn_act_load_kernels"); },

@@ -517,14 +517,28 @@ __global__ void __launch_bounds__(kT, kBwdApplyBlocksPerSM) bn_act_bwd_apply_ker
 // no block synchronisation.  Phase 1 pushes a thread's rows in row order (held rows first, as they come first in the
 // chunk), so the statistics do not depend on how many rows are held.
 //
-// Shared memory of a block, in units of one row-step (kT threads x one unit: kT * V Vec16) with the thread's slot at
-// t * V inside it:
-//   forward    x of held / RL steps | ring: kFwdStages steps of x (with a residual, phase 2 pairs them: x, residual)
-//   backward   dy of held / RL steps | x of them | their mask words | ring: kBwdStages x (dy step, x step, mask words)
-// A mask word is the aligned 4-byte word holding the thread's mask byte (mask_copy).
+// Shared memory of a block: held / RL held row-steps, then the ring (fused_layout).
 constexpr int kResBlocksPerSM = 2;
 constexpr int kFwdStages = 4;
 constexpr int kBwdStages = 2;
+
+// The carve-up of a block's dynamic shared memory, in Vec16: `step` per held row-step and `slot` per ring slot.  A
+// row-step is kT threads x one unit (kT * V Vec16, V Vec16 per unit), the thread's part at t * V; a block of kT mask
+// words (kT / 4 Vec16) holds, at word t, the aligned 4-byte word with the thread's mask byte (mask_copy).
+//   forward              held step: x                   slot: x (with a residual, phase 2 pairs slots: x, residual)
+//   backward             held step: dy, x, mask words   slot: dy, x, mask words
+//   backward, residual   held step: dz, x               slot: dy, dy2, x, mask words (phase 2 uses its dz, x part)
+// The residual backward passes every row through the ring in phase 1, so it always has one.  The kernels index
+// shared memory and fused_plan sizes it from this one function.
+struct Layout {
+  int step, slot;
+  bool ring_always;
+};
+__host__ __device__ constexpr Layout fused_layout(bool bwd, bool res, int V) {
+  return !bwd ? Layout{kT * V, kT * V, false}
+         : !res ? Layout{2 * kT * V + kT / 4, 2 * kT * V + kT / 4, false}
+                : Layout{2 * kT * V, 3 * kT * V + kT / 4, true};
+}
 
 __device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
   uint32_t v;
@@ -616,6 +630,7 @@ __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_fwd_fused_kernel(
     const float* weight, const float* bias, void* y, uint8_t* mask, float* ws, uint32_t* counters) {
   extern __shared__ Vec16 hold[];
   constexpr int V = Unit<U>::kVecs, SV = kT * V;   // SV: Vec16 of one row-step
+  constexpr Layout L = fused_layout(false, kRes, V);
   __shared__ float s_mu[kMaxRedCh], s_sc[kMaxRedCh];
   const int units = C / kCh, CB = 1 << shift, RL = kT >> shift;
   const int col = threadIdx.x & (CB - 1), lane = threadIdx.x >> shift;
@@ -626,8 +641,9 @@ __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_fwd_fused_kernel(
   const int hn = lane < nh ? (nh - 1 - lane) / RL + 1 : 0;
   const int sn = lane < rows - nh ? (rows - nh - 1 - lane) / RL + 1 : 0;
   const size_t i_h = (r0 + lane) * units + u, i_s = i_h + (size_t)nh * units, ustep = (size_t)RL * units;
-  Vec16* hx = hold + threadIdx.x * V;                                  // held step k at hx + k * SV
-  Vec16* ring = hold + (size_t)(held / RL) * SV + threadIdx.x * V;     // ring slot j at ring + j * SV
+  static_assert(L.step == SV && L.slot == SV, "the forward indexes held steps and ring slots of one row-step");
+  Vec16* hx = hold + threadIdx.x * V;                                      // held step k at hx + k * SV
+  Vec16* ring = hold + (size_t)(held / RL) * L.step + threadIdx.x * V;     // ring slot j at ring + j * SV
 
   // phase 1: Welford over the thread's rows in row order, the held ones copied to shared memory on the way
   float n = 0.f, mean[kCh], m2[kCh];
@@ -723,15 +739,28 @@ __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_fwd_fused_kernel(
   }
 }
 
-// Dynamic shared memory: dy, x and the mask words of `held` block rows, then the ring (see above).
+// Dynamic shared memory: `held` block rows, then the ring (fused_layout).
+//
+// Without a residual, phase 1 copies dy, x and the mask word of the held rows to shared memory and streams the
+// rest through the ring; phase 2 applies the held rows from there and streams the others again.
+//
+// With a residual (kRes), phase 1 passes every row through the ring in row order and forms the gradient at the
+// junction, dz = round(dy + dy2) * mask (dy2: the optional second gradient, summed in fp32 and rounded once to the
+// activation dtype as torch's add does).  It writes dz to dres for every row, and a held row keeps dz and x in shared
+// memory.  Phase 2 reads dz back from dres, with x, for the streamed rows: a re-read of two tensors instead of dy,
+// dy2 and the mask.
 template <class U, bool kRelu, bool kRes>
 __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_bwd_fused_kernel(
-    const void* __restrict__ dy, const void* __restrict__ x, const uint8_t* __restrict__ mask, size_t M, int C,
-    int shift, size_t rpc, int held, const float* mean, const float* invstd, const float* weight, float* dweight,
-    float* dbias, void* dx, void* dres, float* ws, uint32_t* counters) {
+    const void* __restrict__ dy, const void* __restrict__ dy2, const void* __restrict__ x,
+    const uint8_t* __restrict__ mask, size_t M, int C, int shift, size_t rpc, int held, const float* mean,
+    const float* invstd, const float* weight, float* dweight, float* dbias, void* dx, void* dres, float* ws,
+    uint32_t* counters) {
   extern __shared__ Vec16 hold[];
-  // SV: Vec16 of one row-step of dy or x; RS: of one ring slot (dy, x, then kT mask words)
-  constexpr int V = Unit<U>::kVecs, SV = kT * V, RS = 2 * SV + kT / 4;
+  // SV: Vec16 of one row-step of dy or x; MW: offset of the mask words in a non-residual held step or ring slot
+  constexpr int V = Unit<U>::kVecs, SV = kT * V, MW = 2 * SV;
+  constexpr Layout L = fused_layout(true, kRes, V);
+  static_assert(kRes || (L.step == MW + kT / 4 && L.slot == L.step), "dy, x, mask words");
+  static_assert(!kRes || (L.step == 2 * SV && L.slot == 3 * SV + kT / 4), "dz, x | dy, dy2, x, mask words");
   __shared__ float s_A[kMaxRedCh], s_D[kMaxRedCh], s_E[kMaxRedCh];
   const int units = C / kCh, CB = 1 << shift, RL = kT >> shift;
   const int col = threadIdx.x & (CB - 1), lane = threadIdx.x >> shift;
@@ -740,32 +769,27 @@ __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_bwd_fused_kernel(
   const int rows = (int)(r1 - r0), nh = min(held, rows);
   const int hn = lane < nh ? (nh - 1 - lane) / RL + 1 : 0;
   const int sn = lane < rows - nh ? (rows - nh - 1 - lane) / RL + 1 : 0;
+  // row-step k of the thread (held ones first) is unit i_h + k * ustep; the streamed ones start at i_s
   const size_t i_h = (r0 + lane) * units + u, i_s = i_h + (size_t)nh * units, ustep = (size_t)RL * units;
   const size_t nm = M * units;
   const int t = threadIdx.x;
   const size_t hs = (size_t)(held / RL);
-  Vec16* hdy = hold + t * V;                                            // held step k at hdy + k * SV, x likewise
-  Vec16* hx = hdy + hs * SV;
-  uint32_t* hm = reinterpret_cast<uint32_t*>(hold + 2 * hs * SV) + t;   // its mask word at hm + k * kT
-  Vec16* ring = hold + hs * (2 * SV + kT / 4);                          // ring slot j at ring + j * RS
-  auto slot_dy = [&](int j) { return ring + j * RS + t * V; };
-  auto slot_x = [&](int j) { return ring + j * RS + SV + t * V; };
-  auto slot_m = [&](int j) { return reinterpret_cast<uint32_t*>(ring + j * RS + 2 * SV) + t; };
-  auto issue_at = [&](int j, size_t i) {
-    hold_copy<U>(slot_dy(j), dy, i);
-    hold_copy<U>(slot_x(j), x, i);
-    if constexpr (kRelu) mask_copy(slot_m(j), mask, i, nm);
+  Vec16* hst = hold + t * V;               // the thread's part of held step k at hst + k * L.step
+  Vec16* ring = hold + hs * L.step + t * V;   // of ring slot j at ring + j * L.slot
+  // the thread's mask word in a step or slot whose mask words start `off` Vec16 into it (p: the thread's part)
+  auto word = [&](Vec16* p, int off) { return reinterpret_cast<uint32_t*>(p - t * V + off) + t; };
+  auto issue_at = [&](int j, size_t i) {   // non-residual ring slot: dy, x, mask word
+    Vec16* s = ring + j * L.slot;
+    hold_copy<U>(s, dy, i);
+    hold_copy<U>(s + SV, x, i);
+    if constexpr (kRelu) mask_copy(word(s, MW), mask, i, nm);
   };
 
-  // phase 1: the thread's rows in row order, the held ones copied to shared memory on the way
+  // phase 1: the thread's rows in row order
   float sg[kCh], sgx[kCh], mu[kCh];
 #pragma unroll
   for (int k = 0; k < kCh; ++k) sg[k] = sgx[k] = 0.f;
-  auto push = [&](const Vec16* pd, const Vec16* px, uint32_t bits) {
-    float d[kCh], f[kCh];
-    hold_load<U>(pd, d);
-    hold_load<U>(px, f);
-    mask_grad<kRelu>(d, bits);
+  auto push = [&](const float* d, const float* f) {
 #pragma unroll
     for (int k = 0; k < kCh; ++k) {
       sg[k] += d[k];
@@ -775,22 +799,72 @@ __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_bwd_fused_kernel(
   if (u < units) {
 #pragma unroll
     for (int k = 0; k < kCh; ++k) mu[k] = mean[u * kCh + k];
-    for (int k = 0; k < hn; ++k) {
-      const size_t i = i_h + k * ustep;
-      hold_copy<U>(hdy + (size_t)k * SV, dy, i);
-      hold_copy<U>(hx + (size_t)k * SV, x, i);
-      if constexpr (kRelu) mask_copy(hm + (size_t)k * kT, mask, i, nm);
+    if constexpr (kRes) {
+      // ring slot: dy, dy2, x, then the mask words at 3 * SV
+      auto issue = [&](int k, int slot) {
+        const size_t i = i_h + k * ustep;
+        Vec16* s = ring + slot * L.slot;
+        hold_copy<U>(s, dy, i);
+        if (dy2 != nullptr) hold_copy<U>(s + SV, dy2, i);
+        hold_copy<U>(s + 2 * SV, x, i);
+        if constexpr (kRelu) mask_copy(word(s, 3 * SV), mask, i, nm);
+      };
+      const int n1 = hn + sn;
+      ring_fill<kBwdStages>(n1, issue);
+      ring_drain<kBwdStages>(n1, issue, [&](int k, int slot) {
+        const size_t i = i_h + k * ustep;
+        Vec16* s = ring + slot * L.slot;
+        float d[kCh], f[kCh];
+        hold_load<U>(s, d);
+        if (dy2 != nullptr) {
+          float e[kCh];
+          hold_load<U>(s + SV, e);
+#pragma unroll
+          for (int c = 0; c < kCh; ++c) d[c] += e[c];
+        }
+        if constexpr (kRelu) mask_grad<kRelu>(d, mask_byte(*word(s, 3 * SV), mask, i));
+        Vec16 z[V], xv[V];
+#pragma unroll
+        for (int v = 0; v < V; ++v) {
+          z[v] = U::pack(d + v * U::kPerVec);   // the rounding of torch's add; exact when there is no dy2
+          U::unpack(z[v], d + v * U::kPerVec);
+          st_stream16(reinterpret_cast<Vec16*>(dres) + i * V + v, z[v]);
+          xv[v] = lds16(s + 2 * SV + v);
+          U::unpack(xv[v], f + v * U::kPerVec);
+        }
+        push(d, f);
+        if (k < hn) {
+          Vec16* h = hst + (size_t)k * L.step;
+#pragma unroll
+          for (int v = 0; v < V; ++v) {
+            sts16(h + v, z[v]);
+            sts16(h + SV + v, xv[v]);
+          }
+        }
+      });
+    } else {
+      // held rows copied to shared memory on the way
+      for (int k = 0; k < hn; ++k) {
+        const size_t i = i_h + k * ustep;
+        Vec16* h = hst + (size_t)k * L.step;
+        hold_copy<U>(h, dy, i);
+        hold_copy<U>(h + SV, x, i);
+        if constexpr (kRelu) mask_copy(word(h, MW), mask, i, nm);
+      }
+      cp_async_commit();
+      auto issue = [&](int k, int slot) { issue_at(slot, i_s + k * ustep); };
+      ring_fill<kBwdStages>(sn, issue);
+      cp_async_wait<kBwdStages>();
+      auto push_smem = [&](Vec16* p, size_t i) {
+        float d[kCh], f[kCh];
+        hold_load<U>(p, d);
+        hold_load<U>(p + SV, f);
+        if constexpr (kRelu) mask_grad<kRelu>(d, mask_byte(*word(p, MW), mask, i));
+        push(d, f);
+      };
+      for (int k = 0; k < hn; ++k) push_smem(hst + (size_t)k * L.step, i_h + k * ustep);
+      ring_drain<kBwdStages>(sn, issue, [&](int k, int slot) { push_smem(ring + slot * L.slot, i_s + k * ustep); });
     }
-    cp_async_commit();
-    auto issue = [&](int k, int slot) { issue_at(slot, i_s + k * ustep); };
-    ring_fill<kBwdStages>(sn, issue);
-    cp_async_wait<kBwdStages>();
-    for (int k = 0; k < hn; ++k)
-      push(hdy + (size_t)k * SV, hx + (size_t)k * SV,
-           kRelu ? mask_byte(hm[(size_t)k * kT], mask, i_h + k * ustep) : 0u);
-    ring_drain<kBwdStages>(sn, issue, [&](int k, int slot) {
-      push(slot_dy(slot), slot_x(slot), kRelu ? mask_byte(*slot_m(slot), mask, i_s + k * ustep) : 0u);
-    });
   }
   tree_sum2<kCh>(sg, sgx, lane, CB, RL);
   const int G = gridDim.x;
@@ -829,7 +903,6 @@ __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_bwd_fused_kernel(
   __syncthreads();
   if (u >= units) return;
 
-  // phase 2
   float A[kCh], D[kCh], E[kCh];
 #pragma unroll
   for (int k = 0; k < kCh; ++k) {
@@ -837,24 +910,34 @@ __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_bwd_fused_kernel(
     D[k] = s_D[col * kCh + k];
     E[k] = s_E[col * kCh + k];
   }
-  // phase 2: streamed rows through the ring, last read first, then the held rows
+  // phase 2: streamed rows through the ring, last read first, then the held rows.  With a residual a slot carries
+  // dz (read back from dres) and x, and the held rows hold dz: the mask is already applied.
   auto unit2 = [&](int k) { return i_s + (size_t)(sn - 1 - k) * ustep; };
-  auto issue2 = [&](int k, int slot) { issue_at(slot, unit2(k)); };
+  auto issue2 = [&](int k, int slot) {
+    if constexpr (kRes) {
+      // This thread stored dres at unit i itself in phase 1, before group_barrier, with a store that does not
+      // allocate in L1; the copy below is issued after it in program order, to the same address, and reads through
+      // L2 (cp.async.cg), so it returns what the thread stored.  No other thread writes this unit.
+      const size_t i = unit2(k);
+      Vec16* s = ring + slot * L.slot;
+      hold_copy<U>(s, dres, i);
+      hold_copy<U>(s + SV, x, i);
+    } else {
+      issue_at(slot, unit2(k));
+    }
+  };
+  auto apply = [&](Vec16* p, size_t i) {
+    float d[kCh], f[kCh];
+    hold_load<U>(p, d);
+    hold_load<U>(p + SV, f);
+    if constexpr (kRes)
+      bwd_row<U, false, false>(i, mu, A, D, E, dx, nullptr, d, f, 0u);
+    else
+      bwd_row<U, kRelu, false>(i, mu, A, D, E, dx, nullptr, d, f, kRelu ? mask_byte(*word(p, MW), mask, i) : 0u);
+  };
   ring_fill<kBwdStages>(sn, issue2);
-  ring_drain<kBwdStages>(sn, issue2, [&](int k, int slot) {
-    const size_t i = unit2(k);
-    float d[kCh], f[kCh];
-    hold_load<U>(slot_dy(slot), d);
-    hold_load<U>(slot_x(slot), f);
-    bwd_row<U, kRelu, kRes>(i, mu, A, D, E, dx, dres, d, f, kRelu ? mask_byte(*slot_m(slot), mask, i) : 0u);
-  });
-  for (int k = 0; k < hn; ++k) {
-    const size_t i = i_h + k * ustep;
-    float d[kCh], f[kCh];
-    hold_load<U>(hdy + (size_t)k * SV, d);
-    hold_load<U>(hx + (size_t)k * SV, f);
-    bwd_row<U, kRelu, kRes>(i, mu, A, D, E, dx, dres, d, f, kRelu ? mask_byte(hm[(size_t)k * kT], mask, i) : 0u);
-  }
+  ring_drain<kBwdStages>(sn, issue2, [&](int k, int slot) { apply(ring + slot * L.slot, unit2(k)); });
+  for (int k = 0; k < hn; ++k) apply(hst + (size_t)k * L.step, i_h + k * ustep);
 }
 
 // ---- synchronised batch norm: the cross-rank step between the local reduction and the apply pass -------------
@@ -975,8 +1058,8 @@ int dtype_index(int dtype) { return dtype == WIRE_F32 ? 0 : dtype == WIRE_BF16 ?
 
 using FusedFwd = void (*)(const void*, const void*, size_t, int, int, size_t, int, float, float, float*, float*,
                           float*, float*, const float*, const float*, void*, uint8_t*, float*, uint32_t*);
-using FusedBwd =void (*)(const void*, const void*, const uint8_t*, size_t, int, int, size_t, int, const float*,
-                          const float*, const float*, float*, float*, void*, void*, float*, uint32_t*);
+using FusedBwd = void (*)(const void*, const void*, const void*, const uint8_t*, size_t, int, int, size_t, int,
+                          const float*, const float*, const float*, float*, float*, void*, void*, float*, uint32_t*);
 
 // Per device: the SM count and, per direction and dtype, the dynamic shared memory a block may hold when
 // kResBlocksPerSM blocks share an SM (0: the single-launch pass cannot run on this device).
@@ -1052,16 +1135,10 @@ struct FusedPlan {
   size_t held_bytes, smem;   // shared memory of the held rows; all dynamic shared memory per block
 };
 
-// Bytes of shared memory per held block row: one unit per thread of dy and x (backward) or x, plus a 4-byte mask
-// word (backward).  A ring stage holds the same for the kT threads of a row-step.
-size_t unit_bytes(int bwd, int dtype) {
-  const size_t vec = (size_t)kCh * (dtype == WIRE_F32 ? 4 : 2);
-  return bwd ? 2 * vec + 4 : vec;
-}
-
-// The whole chunk is held when it fits; otherwise the ring of kFwdStages / kBwdStages row-steps comes first and the
-// held rows get what is left (at most `cap` bytes of them when cap >= 0).
-bool fused_plan(int bwd, int dtype, size_t M, int C, long long cap, FusedPlan* p) {
+// The whole chunk is held when it fits (with the ring the layout always needs); otherwise the ring of kFwdStages /
+// kBwdStages row-steps comes first and the held rows get what is left (at most `cap` bytes of them when cap >= 0).
+// res selects the backward's residual layout (fused_layout).
+bool fused_plan(int bwd, int dtype, size_t M, int C, long long cap, bool res, FusedPlan* p) {
   const int dt = dtype_index(dtype);
   const FusedDev* d = fused_dev();
   if (dt < 0 || bad_shape(M, C) || d == nullptr || d->dyn[bwd ? 1 : 0][dt] == 0) return false;
@@ -1071,33 +1148,34 @@ bool fused_plan(int bwd, int dtype, size_t M, int C, long long cap, FusedPlan* p
   const size_t want = (size_t)(blocks / g.ncb), rl = (size_t)g.rl;
   size_t rpc = (M + want - 1) / want;
   rpc = (rpc < rl ? rl : (rpc + rl - 1) / rl * rl);
+  const Layout L = fused_layout(bwd != 0, bwd && res, dtype == WIRE_F32 ? 2 : 1);
   const size_t dyn = d->dyn[bwd ? 1 : 0][dt], capb = cap >= 0 ? (size_t)cap : dyn;
-  const size_t row = ((size_t)1 << g.shift) * unit_bytes(bwd, dtype);
+  const size_t step = 16 * (size_t)L.step, stages = bwd ? kBwdStages : kFwdStages;   // bytes of a held row-step
   size_t held = rpc;
   int depth = 0;
-  if (rpc * row > (dyn < capb ? dyn : capb)) {
-    depth = bwd ? kBwdStages : kFwdStages;
-    const size_t ring = (size_t)depth * kT * unit_bytes(bwd, dtype);
+  if (L.ring_always || rpc / rl * step > (dyn < capb ? dyn : capb)) {
+    depth = (int)stages;
+    const size_t ring = stages * 16 * (size_t)L.slot;
     if (ring > dyn) return false;
     const size_t budget = dyn - ring < capb ? dyn - ring : capb;
-    held = budget / row / rl * rl;
+    held = budget / step * rl;
+    held = held < rpc ? held : rpc;
   }
-  const size_t hb = held * row;
-  *p = FusedPlan{g, rpc, (int)((M + rpc - 1) / rpc), (int)held, depth, hb,
-                 hb + (size_t)depth * kT * unit_bytes(bwd, dtype)};
+  const size_t hb = held / rl * step;
+  *p = FusedPlan{g, rpc, (int)((M + rpc - 1) / rpc), (int)held, depth, hb, hb + (size_t)depth * 16 * L.slot};
   return true;
 }
 
 // Bytes a launch moves between HBM (or L2) and the SMs: every row once, and the rows a block does not hold again in
-// phase 2 (dy, x and the mask backward; x forward), plus the residual read, the outputs and the mask written.
-size_t fused_bytes(const FusedPlan& p, int bwd, int dtype, size_t M, int C, bool relu, bool res) {
+// phase 2 (x forward; dy, x and the mask backward, or dz and x with a residual), plus the residual or the second
+// gradient (dy2) read, the outputs and the mask written.
+size_t fused_bytes(const FusedPlan& p, int bwd, int dtype, size_t M, int C, bool relu, bool res, bool dy2) {
   const size_t last = M - (size_t)(p.G - 1) * p.rpc;
   const size_t held = (size_t)(p.G - 1) * ((size_t)p.held < p.rpc ? p.held : p.rpc) +
                       ((size_t)p.held < last ? p.held : last);
   const size_t e = (size_t)C * (dtype == WIRE_F32 ? 4 : 2), m = relu ? (size_t)C / kCh : 0;   // per row
-  const size_t reread = (M - held) * (bwd ? 2 * e + m : e);
-  if (bwd) return M * (3 * e + m) + (res ? M * e : 0) + reread;
-  return M * (2 * e + m) + (res ? M * e : 0) + reread;
+  if (bwd) return M * (3 * e + m) + (res ? M * e : 0) + (dy2 ? M * e : 0) + (M - held) * (res ? 2 * e : 2 * e + m);
+  return M * (2 * e + m) + (res ? M * e : 0) + (M - held) * e;
 }
 
 template <class... P, class... A>
@@ -1198,12 +1276,13 @@ cudaError_t launch_bn_act_fwd_stats_local(const void* x, int dtype, size_t M, in
   return cudaGetLastError();
 }
 
-bool bn_act_fused_plan(int bwd, int dtype, size_t M, int C, long long cap, int relu, int residual,
+bool bn_act_fused_plan(int bwd, int dtype, size_t M, int C, long long cap, int relu, int residual, int dy2,
                        BnFusedPlan* out) {
   FusedPlan p;
-  if (!fused_plan(bwd, dtype, M, C, cap, &p)) return false;
+  if (!fused_plan(bwd, dtype, M, C, cap, residual != 0, &p)) return false;
   *out = BnFusedPlan{2 * (size_t)p.G * (size_t)C, p.g.ncb, p.rpc, p.held, p.held_bytes, p.depth, p.smem,
-                     fused_bytes(p, bwd, dtype, M, C, relu != 0, residual != 0), fused_dev()->sms * kResBlocksPerSM};
+                     fused_bytes(p, bwd, dtype, M, C, relu != 0, residual != 0, bwd && residual && dy2),
+                     fused_dev()->sms * kResBlocksPerSM};
   return true;
 }
 
@@ -1215,7 +1294,7 @@ cudaError_t launch_bn_act_fwd(const void* x, const void* residual, int dtype, si
   if (bad_shape(M, C) || M < 2 || !aligned16(x) || !aligned16(residual) || !aligned16(y) ||
       (relu && mask == nullptr) || (running_mean == nullptr) != (running_var == nullptr))
     return cudaErrorInvalidValue;
-  if (!fused_plan(0, dtype, M, C, cap, &p)) return cudaErrorNotSupported;
+  if (!fused_plan(0, dtype, M, C, cap, residual != nullptr, &p)) return cudaErrorNotSupported;
   cudaError_t e = cudaSuccess;
   BN_DISPATCH_U(dtype, BN_DISPATCH_B(relu, kRelu, BN_DISPATCH_B(residual != nullptr, kRes, (
       e = launch_coop(bn_act_fwd_fused_kernel<U, kRelu, kRes>, p, s, x, residual, M, C, p.g.shift, p.rpc, p.held,
@@ -1224,18 +1303,19 @@ cudaError_t launch_bn_act_fwd(const void* x, const void* residual, int dtype, si
   return e;
 }
 
-cudaError_t launch_bn_act_bwd(const void* dy, const void* x, const uint8_t* mask, int dtype, size_t M, int C,
-                              const float* mean, const float* invstd, const float* weight, float* dweight,
+cudaError_t launch_bn_act_bwd(const void* dy, const void* dy2, const void* x, const uint8_t* mask, int dtype, size_t M,
+                              int C, const float* mean, const float* invstd, const float* weight, float* dweight,
                               float* dbias, void* dx, void* dresidual, float* ws, uint32_t* counters, long long cap,
                               cudaStream_t s) {
   FusedPlan p;
-  if (bad_shape(M, C) || !aligned16(dy) || !aligned16(x) || !aligned16(dx) || !aligned16(dresidual))
+  if (bad_shape(M, C) || !aligned16(dy) || !aligned16(dy2) || !aligned16(x) || !aligned16(dx) ||
+      !aligned16(dresidual) || (dy2 != nullptr && dresidual == nullptr))
     return cudaErrorInvalidValue;
-  if (!fused_plan(1, dtype, M, C, cap, &p)) return cudaErrorNotSupported;
+  if (!fused_plan(1, dtype, M, C, cap, dresidual != nullptr, &p)) return cudaErrorNotSupported;
   cudaError_t e = cudaSuccess;
   BN_DISPATCH_U(dtype, BN_DISPATCH_B(mask != nullptr, kRelu, BN_DISPATCH_B(dresidual != nullptr, kRes, (
-      e = launch_coop(bn_act_bwd_fused_kernel<U, kRelu, kRes>, p, s, dy, x, mask, M, C, p.g.shift, p.rpc, p.held,
-                      mean, invstd, weight, dweight, dbias, dx, dresidual, ws, counters)))));
+      e = launch_coop(bn_act_bwd_fused_kernel<U, kRelu, kRes>, p, s, dy, dy2, x, mask, M, C, p.g.shift, p.rpc,
+                      p.held, mean, invstd, weight, dweight, dbias, dx, dresidual, ws, counters)))));
   return e;
 }
 

@@ -46,7 +46,10 @@ cudaError_t launch_bn_act_bwd_apply(const void* dy, const void* x, const uint8_t
 // ---- single-launch passes ------------------------------------------------------------------------------------
 //
 //   fwd   fwd_stats then fwd_apply in one launch: same outputs, save_mean / save_invstd and the running statistics
-//   bwd   bwd_reduce then bwd_apply (dividing by M) in one launch: same outputs, dweight and dbias
+//   bwd   bwd_reduce then bwd_apply (dividing by M) in one launch: same outputs, dweight and dbias.  With a residual it
+//         may take a second gradient dy2 of the output (the gradient of a second consumer, such as a ResNet block's
+//         skip path): it then computes what the two-pass kernels compute for dy + dy2 summed as torch's add does
+//         (in fp32, rounded once to the activation dtype), without that sum ever being stored
 //
 // Each is one cooperative launch of exactly one wave; a grid barrier separates the reduction from the apply.  A block
 // holds its whole chunk in its share of shared memory when it fits; otherwise a ring of a few row-steps streams the
@@ -64,17 +67,19 @@ struct BnFusedPlan {
   size_t held_bytes;       // shared memory of the held rows per block
   int ring_depth;          // row-steps of the streaming ring (0: the whole chunk is held)
   size_t smem_bytes;       // dynamic shared memory per block: held rows and ring
-  size_t bytes_moved;      // bytes a launch with (relu, residual) reads and writes, re-reads of streamed rows included
+  size_t bytes_moved;      // bytes a launch with (relu, residual, dy2) reads and writes, re-reads of streamed rows included
   int wave_blocks;         // blocks in one wave on this device: the grid is at most this large
 };
-bool bn_act_fused_plan(int bwd, int dtype, size_t M, int C, long long cap, int relu, int residual,
+// residual selects the backward's layout too (a residual backward needs more shared memory per ring slot).
+bool bn_act_fused_plan(int bwd, int dtype, size_t M, int C, long long cap, int relu, int residual, int dy2,
                        BnFusedPlan* plan);
 cudaError_t launch_bn_act_fwd(const void* x, const void* residual, int dtype, size_t M, int C, float eps,
                               float momentum, float* running_mean, float* running_var, float* save_mean,
                               float* save_invstd, const float* weight, const float* bias, int relu, void* y,
                               uint8_t* mask, float* ws, uint32_t* counters, long long cap, cudaStream_t s);
-cudaError_t launch_bn_act_bwd(const void* dy, const void* x, const uint8_t* mask, int dtype, size_t M, int C,
-                              const float* mean, const float* invstd, const float* weight, float* dweight,
+// dy2: nullptr, or a second gradient laid out as dy (needs dresidual)
+cudaError_t launch_bn_act_bwd(const void* dy, const void* dy2, const void* x, const uint8_t* mask, int dtype, size_t M,
+                              int C, const float* mean, const float* invstd, const float* weight, float* dweight,
                               float* dbias, void* dx, void* dresidual, float* ws, uint32_t* counters, long long cap,
                               cudaStream_t s);
 

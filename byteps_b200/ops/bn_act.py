@@ -7,6 +7,10 @@ ReLU mask) and one backward (reduce, grid barrier, apply), or two each (the same
 the device cannot run the single-launch kernels at that shape, instead of torch's separate batch-norm, add, ReLU
 and threshold-backward passes.  Every other input - CPU, eval mode, NCHW, C not a multiple of 8 - takes the stock
 ``F.batch_norm`` / add / ``relu`` composition, which computes the same function.
+
+``forward(x, residual, pair=True)`` returns ``(y, alias of y)`` for an output with two consumers (a ResNet block's
+output feeds the next block's conv1 and its skip path).  Autograd then hands backward the two gradients separately,
+and the single-launch backward sums them as it reads them instead of a separate ``add`` pass over the tensor.
 """
 from __future__ import annotations
 
@@ -40,6 +44,13 @@ def _cap() -> int:
     return -1 if RESIDENT_CAP is None else int(RESIDENT_CAP)
 
 
+def _sum_in_kernel(dy, dy2, x) -> bool:
+    """Whether the kernel can read the second gradient beside dy: same dtype as x and dy (so that summing in the
+    kernel rounds as torch's add would), shape of x, channels_last and 16-byte aligned."""
+    return (dy2.dtype == x.dtype and dy.dtype == x.dtype and dy2.shape == x.shape and _nhwc(dy2)
+            and dy2.data_ptr() % 16 == 0)
+
+
 def _workspace(nws, nctr, device):
     return (torch.empty(nws, dtype=torch.float32, device=device),
             torch.zeros(nctr, dtype=torch.int32, device=device))
@@ -47,10 +58,12 @@ def _workspace(nws, nctr, device):
 
 class _BatchNormActFn(torch.autograd.Function):
     """Each direction is one single-launch kernel where the device can run it at the input's shape
-    (``bn_act_plan``), and the two-pass kernels otherwise."""
+    (``bn_act_plan``), and the two-pass kernels otherwise.  With ``pair`` the output is ``(y, y.view_as(y))`` and
+    backward receives the gradients of the two separately (None for an alias nobody used); the single-launch
+    backward with a residual sums them in the kernel, every other path sums them in torch first."""
 
     @staticmethod
-    def forward(ctx, x, residual, weight, bias, running_mean, running_var, momentum, eps, relu):
+    def forward(ctx, x, residual, weight, bias, running_mean, running_var, momentum, eps, relu, pair=False):
         cu = _native.cuda()
         n, c, h, w = x.shape
         m = n * h * w
@@ -76,27 +89,34 @@ class _BatchNormActFn(torch.autograd.Function):
         ctx.save_for_backward(x, weight, mean, invstd, mask)
         ctx.has_residual = residual is not None
         ctx.single_launch_fwd = plan is not None
+        if pair:
+            ctx.set_materialize_grads(False)
+            return y, y.view_as(y)
         return y
 
     @staticmethod
-    def backward(ctx, dy):
+    def backward(ctx, dy, dy2=None):
         x, weight, mean, invstd, mask = ctx.saved_tensors
         cu = _native.cuda()
         n, c, h, w = x.shape
         m = n * h * w
         code = _CODES[x.dtype]
-        dy = dy.to(x.dtype).contiguous(memory_format=torch.channels_last)
+        if dy is None:
+            dy, dy2 = dy2, None
         stream = torch.cuda.current_stream(x.device).cuda_stream
         f32 = dict(dtype=torch.float32, device=x.device)
         dweight, dbias = torch.empty(c, **f32), torch.empty(c, **f32)
         dx = torch.empty_like(x)
         dres = torch.empty_like(x) if ctx.has_residual else None
-        plan = cu.bn_act_plan(1, code, m, c, _cap())
+        plan = cu.bn_act_plan(1, code, m, c, _cap(), residual=ctx.has_residual)
+        if dy2 is not None and not (plan is not None and ctx.has_residual and _sum_in_kernel(dy, dy2, x)):
+            dy, dy2 = dy + dy2, None
+        dy = dy.to(x.dtype).contiguous(memory_format=torch.channels_last)
         if plan is not None:
             ws, ctr = _workspace(plan["ws_floats"], plan["counters"], x.device)
             cu.bn_act_bwd(dy.data_ptr(), x.data_ptr(), _ptr(mask), code, m, c, mean.data_ptr(), invstd.data_ptr(),
                           weight.data_ptr(), dweight.data_ptr(), dbias.data_ptr(), dx.data_ptr(), _ptr(dres),
-                          ws.data_ptr(), ctr.data_ptr(), stream, _cap())
+                          ws.data_ptr(), ctr.data_ptr(), stream, _cap(), _ptr(dy2))
         else:
             ws, ctr = _workspace(*cu.bn_act_workspace(m, c), x.device)
             cu.bn_act_bwd_reduce(dy.data_ptr(), x.data_ptr(), _ptr(mask), code, m, c, mean.data_ptr(),
@@ -105,7 +125,7 @@ class _BatchNormActFn(torch.autograd.Function):
             cu.bn_act_bwd_apply(dy.data_ptr(), x.data_ptr(), _ptr(mask), code, m, c, mean.data_ptr(),
                                 invstd.data_ptr(), weight.data_ptr(), dweight.data_ptr(), dbias.data_ptr(),
                                 dx.data_ptr(), _ptr(dres), stream)
-        return dx, dres, dweight, dbias, None, None, None, None, None
+        return dx, dres, dweight, dbias, None, None, None, None, None, None
 
 
 class BatchNormAct2d(nn.BatchNorm2d):
@@ -127,11 +147,13 @@ class BatchNormAct2d(nn.BatchNorm2d):
                 and x.numel() > x.size(1)
                 and (residual is None or (residual.shape == x.shape and residual.dtype == x.dtype and _nhwc(residual))))
 
-    def _fused(self, x, residual, running_mean, running_var, factor):
+    def _fused(self, x, residual, running_mean, running_var, factor, pair=False):
         return _BatchNormActFn.apply(x, residual, self.weight, self.bias, running_mean, running_var, factor, self.eps,
-                                     self.act == "relu")
+                                     self.act == "relu", pair)
 
-    def forward(self, x, residual=None):
+    def forward(self, x, residual=None, pair=False):
+        """``act(batch_norm(x) [+ residual])``; with ``pair``, ``(y, alias of y)`` for two consumers of y (see the
+        module docstring).  Neither tensor of the pair may be modified in place."""
         # statistics bookkeeping exactly as nn.BatchNorm2d.forward
         self._check_input_dim(x)
         factor = 0.0 if self.momentum is None else self.momentum
@@ -143,13 +165,13 @@ class BatchNormAct2d(nn.BatchNorm2d):
         running_mean = self.running_mean if track else None
         running_var = self.running_var if track else None
         if self._fusable(x, residual, batch_stats):
-            return self._fused(x, residual, running_mean, running_var, factor)
+            return self._fused(x, residual, running_mean, running_var, factor, pair)
         y = F.batch_norm(x, running_mean, running_var, self.weight, self.bias, batch_stats, factor, self.eps)
         if residual is not None:
             y = y + residual
         if self.act == "relu":
             y = F.relu(y, inplace=True)
-        return y
+        return (y, y) if pair else y
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -311,19 +333,20 @@ class SyncBatchNormAct2d(BatchNormAct2d):
     def _fusable(self, x, residual, batch_stats):
         return True if self._synced() else super()._fusable(x, residual, batch_stats)
 
-    def _fused(self, x, residual, running_mean, running_var, factor):
+    def _fused(self, x, residual, running_mean, running_var, factor, pair=False):
         if not self._synced():
-            return super()._fused(x, residual, running_mean, running_var, factor)
-        return _SyncBatchNormActFn.apply(x, residual, self.weight, self.bias, running_mean, running_var, factor,
-                                         self.eps, self.act == "relu", self.sync)
+            return super()._fused(x, residual, running_mean, running_var, factor, pair)
+        y = _SyncBatchNormActFn.apply(x, residual, self.weight, self.bias, running_mean, running_var, factor,
+                                      self.eps, self.act == "relu", self.sync)
+        return (y, y) if pair else y   # autograd sums the two gradients
 
-    def forward(self, x, residual=None):
+    def forward(self, x, residual=None, pair=False):
         if self._synced():
             self._check_input_dim(x)
             why = self._unfusable(x, residual)
             if why is not None:
                 raise ValueError("SyncBatchNormAct2d: synchronised training needs a fusable input, but %s" % why)
-        return super().forward(x, residual)
+        return super().forward(x, residual, pair)
 
 
 def convert_sync_batchnorm(module: nn.Module, sync: Optional[SyncBatchNormContext]) -> nn.Module:
