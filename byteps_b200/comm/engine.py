@@ -202,13 +202,7 @@ class PushPullEngine:
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(t.device))
         self.comm_stream.wait_event(ev)
-        src = t
-        if comp.mom is not None and out.data_ptr() != t.data_ptr():
-            # momentum is folded into the gradient in place: never into the caller's input
-            with torch.cuda.stream(self.comm_stream):
-                out.copy_(t)
-            src = out
-        comp.push_pull(src, out, st.average, stream=self.comm_stream)
+        comp.push_pull(t, out, st.average, stream=self.comm_stream)
         self.launches += 1
         st.done_event = torch.cuda.Event()
         st.done_event.record(self.comm_stream)

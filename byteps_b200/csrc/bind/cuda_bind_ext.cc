@@ -101,9 +101,10 @@ void bind_cuda_ext(py::module_& m) {
 
   // ---- compression kernels (pointers are raw device addresses)
   using S = cudaStream_t;
-  m.def("ef_correct", [](uintptr_t g, int dtype, uintptr_t err, float ratio, uintptr_t corrected, size_t n,
-                         uintptr_t acc, uintptr_t s) {
-    chk(launch_ef_correct((const void*)g, dtype, (const float*)err, ratio, (float*)corrected, n, (float*)acc, (S)s),
+  m.def("ef_correct", [](uintptr_t g, int dtype, uintptr_t mom, float mu, uintptr_t err, float ratio,
+                         uintptr_t corrected, size_t n, uintptr_t acc, uintptr_t s) {
+    chk(launch_ef_correct((const void*)g, dtype, (float*)mom, mu, (const float*)err, ratio, (float*)corrected, n,
+                          (float*)acc, (S)s),
         "ef_correct");
   });
   m.def("index_scatter", [](uintptr_t idx, uintptr_t vals, uint32_t k, size_t n, uintptr_t out, int dtype, float mult,
@@ -124,8 +125,5 @@ void bind_cuda_ext(py::module_& m) {
   });
   m.def("cast_scale", [](uintptr_t in, size_t n, uintptr_t out, int dtype, float mult, uintptr_t s) {
     chk(launch_cast_scale((const float*)in, n, (void*)out, dtype, mult, (S)s), "cast_scale");
-  });
-  m.def("nesterov", [](uintptr_t g, int dtype, uintptr_t mom, float mu, size_t n, uintptr_t s) {
-    chk(launch_nesterov((void*)g, dtype, (float*)mom, mu, n, (S)s), "nesterov");
   });
 }

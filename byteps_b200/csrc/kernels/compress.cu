@@ -34,11 +34,16 @@ __device__ __forceinline__ float warp_max(float v) {
 
 // ---------------------------------------------------------------- error-feedback correction + norms
 template <class U>
-__global__ void ef_correct_kernel(const void* g, const float* err, float ratio, float* corrected, size_t n,
-                                  float* acc) {
+__global__ void ef_correct_kernel(const void* g, float* mom, float mu, const float* err, float ratio, float* corrected,
+                                  size_t n, float* acc) {
   float s_abs = 0.f, s_sq = 0.f, s_max = 0.f;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     float v = load_as_float<U>(g, i);
+    if (mom) {   // nesterov in fp32: the user's gradient is only read
+      const float m = mu * mom[i] + v;
+      mom[i] = m;
+      v += mu * m;
+    }
     if (err) v += ratio * err[i];
     corrected[i] = v;
     float a = fabsf(v);
@@ -194,16 +199,6 @@ __global__ void cast_scale_kernel(const float* in, size_t n, void* out, float mu
     U::store1(out, i, in[i] * mult);
 }
 
-template <class U>
-__global__ void nesterov_kernel(void* g, float* m, float mu, size_t n) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    float gv = U::load1(g, i);
-    float mv = mu * m[i] + gv;
-    m[i] = mv;
-    U::store1(g, i, gv + mu * mv);
-  }
-}
-
 #define DISPATCH_U(dtype, STMT)                    \
   switch (dtype) {                                 \
     case 0: { using U = TagF32; STMT; } break;     \
@@ -214,11 +209,11 @@ __global__ void nesterov_kernel(void* g, float* m, float mu, size_t n) {
 
 }  // namespace
 
-cudaError_t launch_ef_correct(const void* g, int dtype, const float* err, float ratio, float* corrected, size_t n,
-                              float* acc, cudaStream_t s) {
+cudaError_t launch_ef_correct(const void* g, int dtype, float* mom, float mu, const float* err, float ratio,
+                              float* corrected, size_t n, float* acc, cudaStream_t s) {
   // acc layout: [0..3] results, then 3 floats per block (kEfAccFloats in total)
   const int grid = grid_for(n);
-  DISPATCH_U(dtype, (ef_correct_kernel<U><<<grid, kThreads, 0, s>>>(g, err, ratio, corrected, n, acc)));
+  DISPATCH_U(dtype, (ef_correct_kernel<U><<<grid, kThreads, 0, s>>>(g, mom, mu, err, ratio, corrected, n, acc)));
   ef_finalize_kernel<<<1, kThreads, 0, s>>>(acc, grid);
   return cudaGetLastError();
 }
@@ -248,11 +243,6 @@ cudaError_t launch_dither_unpack(const int8_t* levels, const float* scale, size_
 
 cudaError_t launch_cast_scale(const float* in, size_t n, void* out, int dtype, float mult, cudaStream_t s) {
   DISPATCH_U(dtype, (cast_scale_kernel<U><<<grid_for(n), kThreads, 0, s>>>(in, n, out, mult)));
-  return cudaGetLastError();
-}
-
-cudaError_t launch_nesterov(void* g, int dtype, float* m, float mu, size_t n, cudaStream_t s) {
-  DISPATCH_U(dtype, (nesterov_kernel<U><<<grid_for(n), kThreads, 0, s>>>(g, m, mu, n)));
   return cudaGetLastError();
 }
 

@@ -5,7 +5,7 @@
 // the symmetric arena by the kernels of compress_fused.cu (launch_payload_push, then a sum over the
 // local slots).  This file holds the stages those kernels do not fuse: the error-feedback
 // correction (with bit-reproducible norms), the dithering quantiser and unpacker, the random-k
-// scatter, the cast to the user dtype and nesterov momentum.
+// scatter and the cast to the user dtype.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -14,12 +14,13 @@ namespace bps {
 
 // user dtype codes follow WireDType (0 f32, 1 bf16, 2 f16)
 
-// corrected = g + ratio*err (fp32, written to `corrected`); acc[0] = sum|corrected|, acc[1] = sum corrected^2,
-// acc[2] = max|corrected|, computed with a fixed reduction order (bit-reproducible on every rank).
+// corrected = g (+ nesterov momentum) + ratio*err (fp32, written to `corrected`); acc[0] = sum|corrected|,
+// acc[1] = sum corrected^2, acc[2] = max|corrected|, computed with a fixed reduction order (bit-reproducible on
+// every rank).  Momentum (mom non-null, fp32): m = mu*m + g ; corrected = g + mu*m, so g is only read.
 // acc must hold kEfAccFloats floats (results + per-block partials).  err may be null (ratio ignored).
 constexpr int kEfAccFloats = 4 + 3 * 132 * 8;
-cudaError_t launch_ef_correct(const void* g, int dtype, const float* err, float ratio, float* corrected, size_t n,
-                              float* acc, cudaStream_t s);
+cudaError_t launch_ef_correct(const void* g, int dtype, float* mom, float mu, const float* err, float ratio,
+                              float* corrected, size_t n, float* acc, cudaStream_t s);
 
 // ---- random-k
 // out (zeroed by this call) [idx[j]] = mult * vals[j]   (later duplicates win, like the reference)
@@ -37,8 +38,5 @@ cudaError_t launch_dither_unpack(const int8_t* levels, const float* scale, size_
 
 // out = mult * in (fp32 -> user dtype)
 cudaError_t launch_cast_scale(const float* in, size_t n, void* out, int dtype, float mult, cudaStream_t s);
-
-// momentum (nesterov): m = mu*m + g ; g += mu*m   (g in user dtype, m fp32)
-cudaError_t launch_nesterov(void* g, int dtype, float* m, float mu, size_t n, cudaStream_t s);
 
 }  // namespace bps

@@ -290,7 +290,10 @@ struct TopkScratch {
   uint32_t k;
   uint32_t t_lo;     // keys <= t_lo are not histogrammed at level 0 (sampled lower bound of the k-th largest key)
   uint32_t failed;   // the filtered level-0 histogram held fewer than k keys: redo it unfiltered
-  uint32_t pad[7];
+  uint32_t n_tie;    // keys equal to the k-th largest key
+  uint32_t thr;      // the k-th largest key, once the three key levels are done
+  uint32_t k_eq;     // how many of the n_tie ties are kept: the lowest indices (prefix then holds the index cut)
+  uint32_t pad[4];
   uint32_t sample[32768];   // |x| keys of the strided sample (topk_sample_*)
 };
 static_assert(sizeof(TopkScratch) == kTopkScratchBytes, "TopkScratch layout");
@@ -302,7 +305,7 @@ __device__ __forceinline__ void topk_level(int level, int* shift, int* bins) {
 }
 
 // executed by every thread of ONE block once the global histogram of `level` is complete
-__device__ void topk_pick(TopkScratch* sc, int level) {
+__device__ void topk_pick(TopkScratch* sc, int level, bool last_key_level = false) {
   __shared__ uint32_t s_cnt[kT];
   __shared__ uint32_t s_found[3];
   int shift, bins;
@@ -350,6 +353,7 @@ __device__ void topk_pick(TopkScratch* sc, int level) {
     sc->prefix |= (uint32_t)b << shift;
     sc->mask |= (uint32_t)(bins - 1) << shift;
     sc->k_rem = k - cum;
+    if (last_key_level) sc->n_tie = __ldcg(&sc->hist[b]);
   }
   __syncthreads();
   for (int b = t; b < bins; b += kT) sc->hist[b] = 0;
@@ -410,6 +414,40 @@ __global__ void __launch_bounds__(kT) topk_hist_kernel(const float* x, size_t n,
       const uint32_t key = __float_as_uint(p[q]) & 0x7fffffffu;
       if (i + q < n && (key & mask) == prefix && key >= t_lo)
         atomicAdd(&sh_hist[(key >> shift) & (uint32_t)(bins - 1)], 1u);
+    }
+  }
+  hist_flush(sh_hist, sc, bins);
+  if (last_block(&sc->counter)) topk_pick(sc, level, level == 2);
+}
+
+// Ties at the threshold are broken by index, lowest first, so that every rank that selects from the same tensor
+// keeps the same entries: three more radix levels over the key (2^31 - 1 - i) of the tied elements pick the
+// index cut.  A no-op when every tie is kept.
+__device__ __forceinline__ uint32_t tie_key(size_t i) { return 0x7fffffffu - (uint32_t)i; }
+__global__ void topk_tie_init_kernel(TopkScratch* sc) {
+  sc->thr = sc->prefix;
+  sc->k_eq = sc->k_rem;
+  sc->prefix = 0;
+  sc->mask = 0;
+}
+__global__ void __launch_bounds__(kT) topk_tie_hist_kernel(const float* x, size_t n, int level, TopkScratch* sc) {
+  __shared__ uint32_t sh_hist[kTopkBins];
+  if (sc->k_eq == sc->n_tie) return;
+  int shift, bins;
+  topk_level(level, &shift, &bins);
+  for (int b = threadIdx.x; b < bins; b += kT) sh_hist[b] = 0;
+  __syncthreads();
+  const uint32_t thr = sc->thr, prefix = sc->prefix, mask = sc->mask;
+  const size_t n4 = (n + 3) / 4;
+  for (size_t v = (size_t)blockIdx.x * kT + threadIdx.x; v < n4; v += (size_t)gridDim.x * kT) {
+    const size_t i = v * 4;
+    float p[4];
+    loadf4(x, i, n, p);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const uint32_t key = __float_as_uint(p[q]) & 0x7fffffffu, tk = tie_key(i + q);
+      if (i + q < n && key == thr && (tk & mask) == prefix)
+        atomicAdd(&sh_hist[(tk >> shift) & (uint32_t)(bins - 1)], 1u);
     }
   }
   hist_flush(sh_hist, sc, bins);
@@ -525,8 +563,10 @@ __global__ void __launch_bounds__(kT) topk_compact_kernel(float* x, size_t n, ui
                                                           TopkScratch* sc) {
   __shared__ uint32_t s_warp[kT / 32];
   __shared__ uint32_t s_base;
-  const uint32_t thr = sc->prefix, k_eq = sc->k_rem, k = sc->k;
+  const uint32_t thr = sc->thr, k_eq = sc->k_eq, k = sc->k;
   const uint32_t base_eq = k - k_eq;
+  const bool all_ties = k_eq == sc->n_tie;
+  const uint32_t cut = sc->prefix;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const size_t n4 = (n + 3) / 4;
   const size_t per_iter = (size_t)gridDim.x * kT;
@@ -542,7 +582,7 @@ __global__ void __launch_bounds__(kT) topk_compact_kernel(float* x, size_t n, ui
       const uint32_t key = __float_as_uint(p[q]) & 0x7fffffffu;
       const bool live = v < n4 && i + q < n;
       if (live && key > thr) gt_mask |= 1u << q;
-      if (live && key == thr) eq_mask |= 1u << q;
+      if (live && key == thr && (all_ties || tie_key(i + q) >= cut)) eq_mask |= 1u << q;
     }
     // exclusive prefix of the per-thread counts inside the block
     const uint32_t cnt = (uint32_t)__popc(gt_mask);
@@ -574,7 +614,7 @@ __global__ void __launch_bounds__(kT) topk_compact_kernel(float* x, size_t n, ui
         my = slot++;
         take = my < base_eq;
       } else if ((eq_mask & (1u << q)) && k_eq) {
-        const uint32_t e = atomicAdd(&sc->cnt_eq, 1u);        // ties are rare: at most a handful per tensor
+        const uint32_t e = atomicAdd(&sc->cnt_eq, 1u);        // exactly k_eq ties reach here
         if (e < k_eq) {
           my = base_eq + e;
           take = true;
@@ -867,7 +907,7 @@ cudaError_t launch_topk_pre(const void* g, int dtype, float* mom, float mu, cons
 
 cudaError_t launch_topk_finish(float* x, size_t n, uint32_t k, int first_level, uint32_t* pairs, int zero_kept,
                                void* scratch, cudaStream_t s) {
-  if (k == 0 || k > n) return cudaErrorInvalidValue;
+  if (k == 0 || k > n || n > 0x7fffffffu) return cudaErrorInvalidValue;
   TopkScratch* sc = (TopkScratch*)scratch;
   const int grid = grid_for((n + 3) / 4, kFusedMaxBlocks);
   if (first_level == 0) {
@@ -879,6 +919,8 @@ cudaError_t launch_topk_finish(float* x, size_t n, uint32_t k, int first_level, 
     first_level = 1;
   }
   for (int level = first_level; level < 3; ++level) topk_hist_kernel<<<grid, kT, 0, s>>>(x, n, level, 0, sc);
+  topk_tie_init_kernel<<<1, 1, 0, s>>>(sc);
+  for (int level = 0; level < 3; ++level) topk_tie_hist_kernel<<<grid, kT, 0, s>>>(x, n, level, sc);
   topk_compact_kernel<<<grid, kT, 0, s>>>(x, n, pairs, zero_kept, sc);
   return cudaGetLastError();
 }

@@ -239,16 +239,14 @@ class GpuCompressor:
         cor, acc, sm = self.corrected.data_ptr(), self.acc.data_ptr(), self.sum.data_ptr()
 
         def pre():
-            if self.mom is not None:
-                cu.nesterov(g, self.code, mom, mu, n, s)
-            cu.ef_correct(g, self.code, err, ratio, cor, n, acc, s)
+            cu.ef_correct(g, self.code, mom, mu, err, ratio, cor, n, acc, s)
             cu.dither_quantize(cor, n, acc, self.s, self.partition, self.normalize, self.seed, step, pay,
                                pay + self.lv_bytes, err, s)
 
         def post():
             cu.dither_sum_slots(slots, self.slot_bytes, world, n, self.s, self.partition, sm, s)
             if self.two_stage:
-                cu.ef_correct(sm, 0, e2, 1.0, cor, n, acc, s)
+                cu.ef_correct(sm, 0, 0, 0.0, e2, 1.0, cor, n, acc, s)
                 cu.dither_quantize(cor, n, acc, self.s, self.partition, self.normalize, self.seed ^ 0x5555, step,
                                    self.levels2.data_ptr(), self.scale2.data_ptr(), e2, s)
                 cu.dither_unpack(self.levels2.data_ptr(), self.scale2.data_ptr(), n, self.s, self.partition,

@@ -27,10 +27,7 @@ import types
 import pytest
 import torch
 
-F32, BF16, F16 = torch.float32, torch.bfloat16, torch.float16
-DT = {"f32": F32, "bf16": BF16, "f16": F16}
-UNIT = {BF16: 2.0 ** -8, F16: 2.0 ** -11, F32: 2.0 ** -24}
-HALF_MIN_SUB = {BF16: 2.0 ** -134, F16: 2.0 ** -25, F32: 2.0 ** -150}
+from _bounds import BF16, DT, F16, F32, HALF_MIN_SUB, UNIT, stored
 LOSS_SCALE_SUM_LIMIT = 3.38e38       # kLossScaleSumLimit, csrc/kernels/loss_scale.cuh
 GUARD = 4096
 WORLDS = [1, 2, 3, 5, 8]
@@ -101,7 +98,7 @@ def violations(out, e, a, world, c, wire, user=None):
     ok = fin & ~ovf
     b = UNIT[wire] * e.abs() + HALF_MIN_SUB[wire] + c * world * 2.0 ** -24 * a
     if user != wire:
-        b = b + UNIT[user] * (e.abs() + b) + HALF_MIN_SUB[user]
+        b = stored(e.abs(), b, user)
     err = (o - e).abs()
     bad = ok & ~(err <= b)
     bad |= ovf & (o != e.sign() * math.inf)
