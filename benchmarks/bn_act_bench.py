@@ -28,7 +28,19 @@ before.  The stock rows time F.batch_norm [+ add] [+ relu] and its autograd back
 bytes, i.e. they are the rate at which the stock sequence delivers the same work.  Share of peak is against the
 H100 SXM data-sheet 3.35 TB/s; the GPU name and power limit are printed with the table.
 
-    python benchmarks/bn_act_bench.py [--batch 64] [--iters 50] [--rotate-mb 200] [--json out.json]
+The stem rows (64 x 112 x 112, ReLU) compare what the stem ran before the pooled kernels with them.  chain:fwd is
+the single-launch forward then torch's max pool with indices (as autograd runs it); chain:bwd is torch's add of the
+two pooled gradients (the junction before layer1), torch's max-pool backward and the single-launch backward.
+pooled:fwd / pooled:bwd are bn_act_fwd_pool / bn_act_bwd_pool with both gradients.  They report the bytes the
+launches move (the plans' bytes_moved; torch's passes: their tensors once, int64 indices) and the least bytes, P
+pooled rows, M rows, C channels:
+
+    least fwd   read x; write the pooled output and 4-bit codes        M C e + P C (e + 1/2)
+    least bwd   read both pooled gradients, the codes and x; write dx  2 M C e + P C (2 e + 1/2)
+
+with the share of 3.35 TB/s over the least bytes.
+
+    python benchmarks/bn_act_bench.py [--batch 64] [--iters 50] [--rotate-mb 200] [--stem-only] [--json out.json]
 """
 import argparse
 import json
@@ -64,6 +76,7 @@ def main():
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--rotate-mb", type=float, default=200.0, help="bytes the tensor copies of a row span together")
     ap.add_argument("--json", default=None, help="also write the rows as JSON to this file")
+    ap.add_argument("--stem-only", action="store_true", help="only the stem rows (batch norm, ReLU and max pool)")
     args = ap.parse_args()
 
     import torch
@@ -96,7 +109,7 @@ def main():
     print("GPU: %s; batch %d, bf16 activations, fp32 parameters, NHWC" % (info, args.batch))
     print("%-14s %-9s %-11s %9s %9s %8s %6s %9s %7s" % ("C x H x W", "variant", "pass", "MB", "us", "GB/s", "%peak",
                                                        "moved MB", "%peak"))
-    for (c, h, w) in SHAPES:
+    for (c, h, w) in ([] if args.stem_only else SHAPES):
         variants = ["relu"] + (["relu_res", "none"] if (c, h, w) in EXPANDED else [])
         n, m = args.batch * c * h * w, args.batch * h * w
         for var in variants:
@@ -241,6 +254,7 @@ def main():
                     "%dx%dx%d" % (c, h, w), var, row["impl"] + ":" + row["kind"], row["bytes"] / 1e6, row["us"], gbs,
                     100 * row["peak_share"], extra))
             del T, P, XS, RS
+    rows += stem_rows(args, torch, cu, dev, s, timed)
     f_tot = sum(r_["us"] for r_ in rows if r_["impl"] == "fused" and r_["kind"] in ("fwd", "bwd"))
     g_tot = sum(r_["us"] for r_ in rows if r_["impl"] == "single")
     s_tot = sum(r_["us"] for r_ in rows if r_["impl"] == "stock")
@@ -254,6 +268,105 @@ def main():
     if args.json:
         with open(args.json, "w") as fh:
             json.dump({"gpu": info, "batch": args.batch, "rows": rows}, fh, indent=1)
+
+
+def stem_rows(args, torch, cu, dev, s, timed):
+    """The stem's batch norm, ReLU, max pool and pooled junction: the stock chain against the pooled kernels."""
+    c, h, w, e, code = 64, 112, 112, 2, 1
+    oh, ow = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+    m, p = args.batch * h * w, args.batch * oh * ow
+    g = torch.Generator(device=dev).manual_seed(0)
+    nhwc = dict(memory_format=torch.channels_last)
+    k = max(1, int(-(-args.rotate_mb * 1e6 // (m * c * e * 3 + p * c * e * 2))))
+
+    def copies():
+        x = torch.randn(args.batch, c, h, w, device=dev, generator=g).to(torch.bfloat16).contiguous(**nhwc)
+        g1 = torch.randn(args.batch, c, oh, ow, device=dev, generator=g).to(torch.bfloat16).contiguous(**nhwc)
+        return dict(x=x, y=torch.empty_like(x), dx=torch.empty_like(x), g1=g1, g2=torch.randn_like(g1),
+                    pooled=torch.empty_like(g1), mask=torch.empty(m, c // 8, dtype=torch.uint8, device=dev),
+                    code=torch.empty(p, c // 8, dtype=torch.int32, device=dev))
+
+    T = [copies() for _ in range(k)]
+    wt, bs = torch.ones(c, device=dev), torch.zeros(c, device=dev)
+    rm, rv = torch.zeros(c, device=dev), torch.ones(c, device=dev)
+    mean, inv, dw, db = (torch.empty(c, device=dev) for _ in range(4))
+    fplan, bplan = cu.bn_act_plan(0, code, m, c, relu=True), cu.bn_act_plan(1, code, m, c, relu=True)
+    pf = cu.bn_act_plan(0, code, m, c, relu=True, pool_h=h, pool_w=w)
+    pb = cu.bn_act_plan(1, code, m, c, relu=True, dy2=True, pool_h=h, pool_w=w)
+    if None in (fplan, bplan, pf, pb):
+        print("stem: a single-launch plan is refused on this device; no stem rows")
+        return []
+    ws = torch.empty(max(pl["ws_floats"] for pl in (fplan, bplan, pf, pb)), device=dev)
+    ctrs = torch.zeros(2 * (args.iters + max(3, k)), max(pl["counters"] for pl in (fplan, bplan, pf, pb)),
+                       dtype=torch.int32, device=dev)
+    launch = [0]
+
+    def zeroed():
+        launch[0] += 1
+        return ctrs[launch[0] - 1].data_ptr()
+
+    def fwd(i):
+        t = T[i]
+        cu.bn_act_fwd(t["x"].data_ptr(), 0, code, m, c, 1e-5, 0.1, rm.data_ptr(), rv.data_ptr(), mean.data_ptr(),
+                      inv.data_ptr(), wt.data_ptr(), bs.data_ptr(), True, t["y"].data_ptr(), t["mask"].data_ptr(),
+                      ws.data_ptr(), zeroed(), s)
+
+    def chain_fwd(i):
+        fwd(i)
+        T[i]["pool"] = torch.ops.aten.max_pool2d_with_indices(T[i]["y"], [3, 3], [2, 2], [1, 1])
+
+    def chain_bwd(i):
+        t = T[i]
+        gsum = torch.add(t["g1"], t["g2"])
+        dy = torch.ops.aten.max_pool2d_with_indices_backward(gsum, t["y"], [3, 3], [2, 2], [1, 1], [1, 1], False,
+                                                              t["pool"][1])
+        cu.bn_act_bwd(dy.data_ptr(), t["x"].data_ptr(), t["mask"].data_ptr(), code, m, c, mean.data_ptr(),
+                      inv.data_ptr(), wt.data_ptr(), dw.data_ptr(), db.data_ptr(), t["dx"].data_ptr(), 0,
+                      ws.data_ptr(), zeroed(), s)
+
+    def pooled_fwd(i):
+        t = T[i]
+        cu.bn_act_fwd_pool(t["x"].data_ptr(), code, args.batch, h, w, c, 1e-5, 0.1, rm.data_ptr(), rv.data_ptr(),
+                           mean.data_ptr(), inv.data_ptr(), wt.data_ptr(), bs.data_ptr(), t["pooled"].data_ptr(),
+                           t["code"].data_ptr(), ws.data_ptr(), zeroed(), s)
+
+    def pooled_bwd(i):
+        t = T[i]
+        cu.bn_act_bwd_pool(t["g1"].data_ptr(), t["g2"].data_ptr(), t["code"].data_ptr(), t["x"].data_ptr(), code,
+                           args.batch, h, w, c, mean.data_ptr(), inv.data_ptr(), wt.data_ptr(), dw.data_ptr(),
+                           db.data_ptr(), t["dx"].data_ptr(), ws.data_ptr(), zeroed(), s)
+
+    def run(fn):
+        launch[0] = 0
+        ctrs.zero_()
+        return timed(fn, k)
+
+    for i in range(k):   # the chain's indices and the pooled codes the backward rows read
+        chain_fwd(i)
+        pooled_fwd(i)
+    torch.cuda.synchronize()
+    least_f, least_b = m * c * e + p * c * (e + 0.5), 2 * m * c * e + p * c * (2 * e + 0.5)
+    pool_f = m * c * e + p * c * (e + 8)                     # torch's max pool: read y; write the output, indices
+    pool_b = p * c * (e + 8) + m * c * e + 3 * p * c * e      # its backward and the add of the two gradients
+    out = []
+    for impl, kind, fn, moved, least in (
+            ("chain", "fwd", chain_fwd, fplan["bytes_moved"] + pool_f, least_f),
+            ("chain", "bwd", chain_bwd, bplan["bytes_moved"] + pool_b, least_b),
+            ("pooled", "fwd", pooled_fwd, pf["bytes_moved"], least_f),
+            ("pooled", "bwd", pooled_bwd, pb["bytes_moved"], least_b)):
+        us = run(fn) * 1e3
+        out.append(dict(shape=[c, h, w], variant="relu_pool", impl=impl, kind=kind, us=us, bytes=least,
+                        bytes_moved=moved, gbs=least / (us * 1e3), peak_share=least / (us * 1e3) / PEAK_GBS))
+    print("stem %dx%dx%d, batch %d: ReLU, max pool 3 / 2 / 1 and the pooled junction (least MB: forward %.1f, "
+          "backward %.1f)" % (c, h, w, args.batch, least_f / 1e6, least_b / 1e6))
+    print("%-12s %9s %9s %9s %7s" % ("pass", "us", "moved MB", "least MB", "%peak"))
+    for r_ in out:
+        print("%-12s %9.1f %9.1f %9.1f %6.0f%%" % (r_["impl"] + ":" + r_["kind"], r_["us"], r_["bytes_moved"] / 1e6,
+                                                  r_["bytes"] / 1e6, 100 * r_["peak_share"]))
+    us = {(r_["impl"], r_["kind"]): r_["us"] for r_ in out}
+    print("stem: chain -> pooled saves %.0f us per step" % (
+        us[("chain", "fwd")] + us[("chain", "bwd")] - us[("pooled", "fwd")] - us[("pooled", "bwd")]))
+    return out
 
 
 if __name__ == "__main__":

@@ -61,9 +61,10 @@ void bind_cuda_bn(py::module_& m) {
 
   // ---- single-launch passes
   m.def("bn_act_plan", [](int bwd, int dtype, size_t M, int C, long long cap, bool relu, bool residual,
-                          bool dy2) -> py::object {
+                          bool dy2, int pool_h, int pool_w) -> py::object {
     BnFusedPlan p;
-    if (!bn_act_fused_plan(bwd, dtype, M, C, cap, relu ? 1 : 0, residual ? 1 : 0, dy2 ? 1 : 0, &p)) return py::none();
+    if (!bn_act_fused_plan(bwd, dtype, M, C, cap, relu ? 1 : 0, residual ? 1 : 0, dy2 ? 1 : 0, &p, pool_h, pool_w))
+      return py::none();
     py::dict d;
     d["ws_floats"] = p.ws_floats;
     d["counters"] = p.counters;
@@ -76,11 +77,13 @@ void bind_cuda_bn(py::module_& m) {
     d["wave_blocks"] = p.wave_blocks;
     return d;
   }, py::arg("bwd"), py::arg("dtype"), py::arg("M"), py::arg("C"), py::arg("cap") = -1, py::arg("relu") = false,
-     py::arg("residual") = false, py::arg("dy2") = false,
+     py::arg("residual") = false, py::arg("dy2") = false, py::arg("pool_h") = 0, py::arg("pool_w") = 0,
      "plan of the single-launch bn_act_fwd (bwd=0) / bn_act_bwd (bwd=1) at (M, C, dtype) on the current device, or "
      "None when it cannot run there; cap >= 0 limits the bytes of rows a block holds in shared memory.  residual "
      "selects the backward's shared-memory layout; relu, residual and dy2 (a second gradient, backward with a "
-     "residual) select the variant whose bytes_moved is reported");
+     "residual) select the variant whose bytes_moved is reported.  pool_h, pool_w > 0: the pooled passes "
+     "(bn_act_fwd_pool / bn_act_bwd_pool, relu without residual) over images of pool_h x pool_w; dy2 then means a "
+     "second pooled gradient");
   m.def("bn_act_fwd", [](uintptr_t x, uintptr_t residual, int dtype, size_t M, int C, float eps, float momentum,
                          uintptr_t running_mean, uintptr_t running_var, uintptr_t save_mean, uintptr_t save_invstd,
                          uintptr_t weight, uintptr_t bias, bool relu, uintptr_t y, uintptr_t mask, uintptr_t ws,
@@ -108,6 +111,34 @@ void bind_cuda_bn(py::module_& m) {
      py::arg("ws"), py::arg("counters"), py::arg("stream"), py::arg("cap") = -1, py::arg("dy2") = 0,
      "dy2: 0, or a second gradient of the output laid out as dy (M x C, 16-byte aligned; needs dresidual), summed "
      "with dy inside the kernel");
+
+  m.def("bn_act_fwd_pool", [](uintptr_t x, int dtype, int N, int H, int W, int C, float eps, float momentum,
+                              uintptr_t running_mean, uintptr_t running_var, uintptr_t save_mean,
+                              uintptr_t save_invstd, uintptr_t weight, uintptr_t bias, uintptr_t pooled, uintptr_t code,
+                              uintptr_t ws, uintptr_t counters, uintptr_t s, long long cap) {
+    chk(launch_bn_act_fwd_pool((const void*)x, dtype, N, H, W, C, eps, momentum, (float*)running_mean,
+                               (float*)running_var, (float*)save_mean, (float*)save_invstd, (const float*)weight,
+                               (const float*)bias, (void*)pooled, (uint32_t*)code, (float*)ws, (uint32_t*)counters,
+                               cap, (cudaStream_t)s),
+        "bn_act_fwd_pool");
+  }, py::arg("x"), py::arg("dtype"), py::arg("N"), py::arg("H"), py::arg("W"), py::arg("C"), py::arg("eps"),
+     py::arg("momentum"), py::arg("running_mean"), py::arg("running_var"), py::arg("save_mean"),
+     py::arg("save_invstd"), py::arg("weight"), py::arg("bias"), py::arg("pooled"), py::arg("code"), py::arg("ws"),
+     py::arg("counters"), py::arg("stream"), py::arg("cap") = -1,
+     "single-launch batch norm, ReLU and 3x3 / stride 2 / padding 1 max pool: the pooled output (N x OH x OW x C) and "
+     "its window codes (N * OH * OW * C / 8 uint32)");
+  m.def("bn_act_bwd_pool", [](uintptr_t g1, uintptr_t g2, uintptr_t code, uintptr_t x, int dtype, int N, int H, int W,
+                              int C, uintptr_t mean, uintptr_t invstd, uintptr_t weight, uintptr_t dweight,
+                              uintptr_t dbias, uintptr_t dx, uintptr_t ws, uintptr_t counters, uintptr_t s,
+                              long long cap) {
+    chk(launch_bn_act_bwd_pool((const void*)g1, (const void*)g2, (const uint32_t*)code, (const void*)x, dtype, N, H, W,
+                               C, (const float*)mean, (const float*)invstd, (const float*)weight, (float*)dweight,
+                               (float*)dbias, (void*)dx, (float*)ws, (uint32_t*)counters, cap, (cudaStream_t)s),
+        "bn_act_bwd_pool");
+  }, py::arg("g1"), py::arg("g2"), py::arg("code"), py::arg("x"), py::arg("dtype"), py::arg("N"), py::arg("H"),
+     py::arg("W"), py::arg("C"), py::arg("mean"), py::arg("invstd"), py::arg("weight"), py::arg("dweight"),
+     py::arg("dbias"), py::arg("dx"), py::arg("ws"), py::arg("counters"), py::arg("stream"), py::arg("cap") = -1,
+     "backward of bn_act_fwd_pool for the pooled gradients g1 and g2 (0: none), summed as torch's add");
 
   // ---- synchronised batch norm
   m.def("bn_act_load_kernels", []() { chk(bn_act_load_kernels(), "bn_act_load_kernels"); },

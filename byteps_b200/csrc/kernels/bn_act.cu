@@ -74,6 +74,11 @@ struct Unit {
 #pragma unroll
     for (int v = 0; v < kVecs; ++v) st_stream16(p + v, U::pack(f + v * U::kPerVec));
   }
+  // rounds f to the activation dtype, as storing and reloading it would
+  __device__ static __forceinline__ void round(float* f) {
+#pragma unroll
+    for (int v = 0; v < kVecs; ++v) U::unpack(U::pack(f + v * U::kPerVec), f + v * U::kPerVec);
+  }
 };
 
 __device__ __forceinline__ void welford_push(float& n, float* mean, float* m2, const float* f) {
@@ -308,6 +313,9 @@ __global__ void __launch_bounds__(kT, kBlocksPerSM) bn_act_fwd_stats_kernel(cons
   }
 }
 
+// The normalised, scaled and shifted value of x = f before the residual and the activation; every apply forms it so.
+__device__ __forceinline__ float bn_value(float f, float mu, float sc, float sh) { return fmaf(f - mu, sc, sh); }
+
 template <class U, bool kRelu, bool kRes>
 __device__ __forceinline__ void fwd_row(size_t i, const float* mu, const float* sc, const float* sh, void* y,
                                         uint8_t* mask, const float* f, const float* q) {
@@ -315,7 +323,7 @@ __device__ __forceinline__ void fwd_row(size_t i, const float* mu, const float* 
   uint32_t bits = 0;
 #pragma unroll
   for (int k = 0; k < kCh; ++k) {
-    float v = fmaf(f[k] - mu[k], sc[k], sh[k]);
+    float v = bn_value(f[k], mu[k], sc[k], sh[k]);
     if constexpr (kRes) v += q[k];
     if constexpr (kRelu) {
       bits |= (v > 0.f ? 1u : 0u) << k;
@@ -528,14 +536,16 @@ constexpr int kBwdStages = 2;
 //   forward              held step: x                   slot: x (with a residual, phase 2 pairs slots: x, residual)
 //   backward             held step: dy, x, mask words   slot: dy, x, mask words
 //   backward, residual   held step: dz, x               slot: dy, dy2, x, mask words (phase 2 uses its dz, x part)
-// The residual backward passes every row through the ring in phase 1, so it always has one.  The kernels index
-// shared memory and fused_plan sizes it from this one function.
+//   backward, pooled     held step: dyi, x              slot: x (dyi is formed from the pooled gradients)
+// The pooled forward uses the forward's layout.  The residual backward passes every row through the ring in phase 1,
+// so it always has one.  The kernels index shared memory and fused_plan sizes it from this one function.
 struct Layout {
   int step, slot;
   bool ring_always;
 };
-__host__ __device__ constexpr Layout fused_layout(bool bwd, bool res, int V) {
+__host__ __device__ constexpr Layout fused_layout(bool bwd, bool res, int V, bool pool = false) {
   return !bwd ? Layout{kT * V, kT * V, false}
+         : pool ? Layout{2 * kT * V, kT * V, false}
          : !res ? Layout{2 * kT * V + kT / 4, 2 * kT * V + kT / 4, false}
                 : Layout{2 * kT * V, 3 * kT * V + kT / 4, true};
 }
@@ -622,12 +632,55 @@ __device__ __forceinline__ void hold_copy(Vec16* h, const void* base, size_t uni
   for (int v = 0; v < Unit<U>::kVecs; ++v) cp_async16(h + v, p + v);
 }
 
+// ---- the pooled variant: ReLU then max pool (kernel 3, stride 2, padding 1) of the stem
+//
+// Rows are the pixels (n, h, w) of N images of H x W; the pooled rows (n, oh, ow) of OH x OW, OH = (H - 1) / 2 + 1,
+// are ordered the same way, so their window centres (n, 2 oh, 2 ow) increase with the pooled row.  Per unit and
+// pooled row the forward writes one 32-bit code word, 4 bits per channel (bits 4k .. 4k + 3: channel 8j + k): the
+// window position kh * 3 + kw of the channel's maximum, or kPoolDead when that maximum carries no gradient.
+constexpr uint32_t kPoolDead = 0xf;
+
+struct PoolShape {
+  int H, W, OH, OW;
+  size_t hw, ohw;
+  __host__ __device__ PoolShape(int h, int w)
+      : H(h), W(w), OH((h - 1) / 2 + 1), OW((w - 1) / 2 + 1), hw((size_t)h * w),
+        ohw((size_t)((h - 1) / 2 + 1) * ((w - 1) / 2 + 1)) {}
+  // pooled rows whose window centre is a row before r
+  __host__ __device__ size_t pooled_before(size_t r) const {
+    const size_t n = r / hw;
+    const int rem = (int)(r - n * hw), h = rem / W, w = rem - h * W;
+    return n * ohw + (size_t)((h + 1) / 2) * OW + (h % 2 == 0 ? (w + 1) / 2 : 0);
+  }
+  __host__ __device__ void pooled_at(size_t j, size_t* n, int* oh, int* ow) const { split2(j, ohw, OW, n, oh, ow); }
+  __host__ __device__ void split(size_t r, size_t* n, int* h, int* w) const { split2(r, hw, W, n, h, w); }
+  // i = (n * plane + a) * width + b; 32-bit divisions where i fits, as it does at any practical size
+  __host__ __device__ static void split2(size_t i, size_t plane, int width, size_t* n, int* a, int* b) {
+    if ((i | plane) <= 0xffffffffu) {
+      const uint32_t n32 = (uint32_t)i / (uint32_t)plane, rem = (uint32_t)i - n32 * (uint32_t)plane;
+      *n = n32;
+      *a = (int)(rem / (uint32_t)width);
+      *b = (int)(rem - (uint32_t)*a * (uint32_t)width);
+    } else {
+      *n = i / plane;
+      const int rem = (int)(i - *n * plane);
+      *a = rem / width;
+      *b = rem - *a * width;
+    }
+  }
+};
+
 // Dynamic shared memory: x of `held` block rows, then the ring (see above).
-template <class U, bool kRelu, bool kRes>
+//
+// kPool (with kRelu, without kRes): the rows are images of IH x IW, and phase 2 writes the max pool of y to y (pooled
+// rows) and the window codes to pool_code instead of y and the mask; phase 1 is the same as without it.
+template <class U, bool kRelu, bool kRes, bool kPool>
 __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_fwd_fused_kernel(
     const void* __restrict__ x, const void* __restrict__ res, size_t M, int C, int shift, size_t rpc, int held,
     float eps, float momentum, float* run_mean, float* run_var, float* save_mean, float* save_invstd,
-    const float* weight, const float* bias, void* y, uint8_t* mask, float* ws, uint32_t* counters) {
+    const float* weight, const float* bias, void* y, uint8_t* mask, float* ws, uint32_t* counters, int IH, int IW,
+    uint32_t* pool_code) {
+  static_assert(!kPool || (kRelu && !kRes), "the pooled forward is ReLU without a residual");
   extern __shared__ Vec16 hold[];
   constexpr int V = Unit<U>::kVecs, SV = kT * V;   // SV: Vec16 of one row-step
   constexpr Layout L = fused_layout(false, kRes, V);
@@ -707,6 +760,74 @@ __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_fwd_fused_kernel(
     sc[k] = s_sc[col * kCh + k];
     sh[k] = bias[u * kCh + k];
   }
+  if constexpr (kPool) {
+    // The block's pooled outputs: those whose window centre (n, 2 oh, 2 ow) lies in the chunk, a contiguous range
+    // [p0, p1) of the pooled rows, walked in order so that the image lines a step reads are read again by the next
+    // steps while still in L1 / L2.  A window row the block holds comes from shared memory (held row r0 + i of
+    // column col sits at ((i * CB + col) * V), any other, halo rows of the neighbouring chunks included, from global
+    // memory: x is read-only, so no synchronisation is needed.  y is formed as fwd_row forms it and rounded to the
+    // activation dtype; the maximum is picked as torch's NHWC max pool does (window scanned row-major, strict >, a
+    // NaN always taken).  The code of a channel is the winner's window position, or kPoolDead when the winner's
+    // ReLU mask bit would be 0 (y <= 0 before the ReLU), where the stock chain's gradient ends.
+    const PoolShape ps(IH, IW);
+    const size_t p0 = ps.pooled_before(r0), p1 = ps.pooled_before(r1);
+    for (size_t j = p0 + lane; j < p1; j += RL) {
+      size_t n;
+      int oh, ow;
+      ps.pooled_at(j, &n, &oh, &ow);
+      float best[kCh];
+      uint32_t code = 0, live = 0;
+#pragma unroll
+      for (int k = 0; k < kCh; ++k) best[k] = -INFINITY;
+      // QB window positions at a time, their loads in flight together (generic loads: shared or global memory)
+      constexpr int QB = V == 1 ? 9 : 3;
+#pragma unroll
+      for (int q0 = 0; q0 < 9; q0 += QB) {
+        Vec16 raw[QB][V];
+#pragma unroll
+        for (int q = q0; q < q0 + QB; ++q) {
+          const int h = 2 * oh - 1 + q / 3, w = 2 * ow - 1 + q % 3;
+          if (h < 0 || h >= IH || w < 0 || w >= IW) continue;
+          const size_t r = n * ps.hw + (size_t)h * IW + w;
+          const uint4* src = r - r0 < (size_t)nh ? reinterpret_cast<const uint4*>(hold + ((r - r0) * CB + col) * V)
+                                                : reinterpret_cast<const uint4*>(x) + (r * units + u) * V;
+#pragma unroll
+          for (int v = 0; v < V; ++v) {
+            const uint4 t = src[v];
+            raw[q - q0][v] = Vec16{t.x, t.y, t.z, t.w};
+          }
+        }
+#pragma unroll
+        for (int q = q0; q < q0 + QB; ++q) {
+          const int h = 2 * oh - 1 + q / 3, w = 2 * ow - 1 + q % 3;
+          if (h < 0 || h >= IH || w < 0 || w >= IW) continue;
+          float f[kCh], v[kCh], o[kCh];
+#pragma unroll
+          for (int e = 0; e < V; ++e) U::unpack(raw[q - q0][e], f + e * U::kPerVec);
+#pragma unroll
+          for (int k = 0; k < kCh; ++k) {
+            v[k] = bn_value(f[k], mu[k], sc[k], sh[k]);
+            o[k] = v[k] <= 0.f ? 0.f : v[k];   // as fwd_row's ReLU
+          }
+          Unit<U>::round(o);
+#pragma unroll
+          for (int k = 0; k < kCh; ++k) {
+            if (o[k] > best[k] || isnan(o[k])) {
+              best[k] = o[k];
+              code = (code & ~(0xfu << (4 * k))) | (uint32_t)q << (4 * k);
+              live = (live & ~(1u << k)) | (v[k] > 0.f ? 1u : 0u) << k;
+            }
+          }
+        }
+      }
+#pragma unroll
+      for (int k = 0; k < kCh; ++k)
+        if (!((live >> k) & 1u)) code |= kPoolDead << (4 * k);
+      Unit<U>::store(y, j * units + u, best);
+      pool_code[j * units + u] = code;
+    }
+    return;
+  }
   constexpr int W = kRes ? 2 : 1, D2 = kFwdStages / W;
   const int n2 = sn + (kRes && (size_t)held < rpc ? hn : 0);
   auto unit2 = [&](int k) { return k < sn ? i_s + (size_t)(sn - 1 - k) * ustep : i_h + (size_t)(k - sn) * ustep; };
@@ -739,6 +860,60 @@ __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_fwd_fused_kernel(
   }
 }
 
+// Between the phases of a single-launch backward: the block's sums of g and g * (x - mean) (sg, sgx of the thread)
+// are reduced, the channel group's blocks meet at the grid barrier, each merges the G partials in the same fixed
+// order and derives bwd_apply's coefficients dx = A * g + D * (x - mean) + E of the thread's channels; block 0 writes
+// dweight and dbias.  Returns false for a thread without a unit (u >= units), which has nothing left to do.
+__device__ __forceinline__ bool bwd_coefficients(float* sg, float* sgx, int lane, int col, int CB, int RL, int u,
+                                                 int units, size_t M, int C, const float* invstd, const float* weight,
+                                                 float* dweight, float* dbias, float* ws, uint32_t* counters, float* A,
+                                                 float* D, float* E) {
+  __shared__ float s_A[kMaxRedCh], s_D[kMaxRedCh], s_E[kMaxRedCh];
+  tree_sum2<kCh>(sg, sgx, lane, CB, RL);
+  const int G = gridDim.x;
+  if (lane == 0 && u < units) {
+#pragma unroll
+    for (int k = 0; k < kCh; ++k) {
+      ws[(size_t)blockIdx.x * C + u * kCh + k] = sg[k];
+      ws[((size_t)G + blockIdx.x) * C + u * kCh + k] = sgx[k];
+    }
+  }
+  group_barrier(counters + blockIdx.y);
+
+  const Fin fin(CB);
+  const int c = blockIdx.y * fin.nc + fin.cl;
+  float a = 0.f, b = 0.f;
+  if (c < C) {
+#pragma unroll 8
+    for (int g = fin.sub; g < G; g += fin.tpc) {
+      a += __ldcg(ws + (size_t)g * C + c);
+      b += __ldcg(ws + ((size_t)G + g) * C + c);
+    }
+  }
+  tree_sum2<1>(&a, &b, fin.sub, fin.nc, fin.tpc);
+  if (fin.sub == 0 && c < C) {
+    // the coefficients of bwd_apply, from the same sums
+    const float is = invstd[c], db = a, dw = b * is, invM = 1.f / (float)M;
+    const float a_ = weight[c] * is;
+    s_A[fin.cl] = a_;
+    s_D[fin.cl] = -a_ * is * (dw * invM);
+    s_E[fin.cl] = -a_ * (db * invM);
+    if (blockIdx.x == 0) {
+      dbias[c] = db;
+      dweight[c] = dw;
+    }
+  }
+  __syncthreads();
+  if (u >= units) return false;
+#pragma unroll
+  for (int k = 0; k < kCh; ++k) {
+    A[k] = s_A[col * kCh + k];
+    D[k] = s_D[col * kCh + k];
+    E[k] = s_E[col * kCh + k];
+  }
+  return true;
+}
+
 // Dynamic shared memory: `held` block rows, then the ring (fused_layout).
 //
 // Without a residual, phase 1 copies dy, x and the mask word of the held rows to shared memory and streams the
@@ -761,7 +936,6 @@ __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_bwd_fused_kernel(
   constexpr Layout L = fused_layout(true, kRes, V);
   static_assert(kRes || (L.step == MW + kT / 4 && L.slot == L.step), "dy, x, mask words");
   static_assert(!kRes || (L.step == 2 * SV && L.slot == 3 * SV + kT / 4), "dz, x | dy, dy2, x, mask words");
-  __shared__ float s_A[kMaxRedCh], s_D[kMaxRedCh], s_E[kMaxRedCh];
   const int units = C / kCh, CB = 1 << shift, RL = kT >> shift;
   const int col = threadIdx.x & (CB - 1), lane = threadIdx.x >> shift;
   const int u = blockIdx.y * CB + col;
@@ -769,6 +943,7 @@ __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_bwd_fused_kernel(
   const int rows = (int)(r1 - r0), nh = min(held, rows);
   const int hn = lane < nh ? (nh - 1 - lane) / RL + 1 : 0;
   const int sn = lane < rows - nh ? (rows - nh - 1 - lane) / RL + 1 : 0;
+  float A[kCh], D[kCh], E[kCh];
   // row-step k of the thread (held ones first) is unit i_h + k * ustep; the streamed ones start at i_s
   const size_t i_h = (r0 + lane) * units + u, i_s = i_h + (size_t)nh * units, ustep = (size_t)RL * units;
   const size_t nm = M * units;
@@ -866,50 +1041,9 @@ __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_bwd_fused_kernel(
       ring_drain<kBwdStages>(sn, issue, [&](int k, int slot) { push_smem(ring + slot * L.slot, i_s + k * ustep); });
     }
   }
-  tree_sum2<kCh>(sg, sgx, lane, CB, RL);
-  const int G = gridDim.x;
-  if (lane == 0 && u < units) {
-#pragma unroll
-    for (int k = 0; k < kCh; ++k) {
-      ws[(size_t)blockIdx.x * C + u * kCh + k] = sg[k];
-      ws[((size_t)G + blockIdx.x) * C + u * kCh + k] = sgx[k];
-    }
-  }
-  group_barrier(counters + blockIdx.y);
-
-  const Fin fin(CB);
-  const int c = blockIdx.y * fin.nc + fin.cl;
-  float a = 0.f, b = 0.f;
-  if (c < C) {
-#pragma unroll 8
-    for (int g = fin.sub; g < G; g += fin.tpc) {
-      a += __ldcg(ws + (size_t)g * C + c);
-      b += __ldcg(ws + ((size_t)G + g) * C + c);
-    }
-  }
-  tree_sum2<1>(&a, &b, fin.sub, fin.nc, fin.tpc);
-  if (fin.sub == 0 && c < C) {
-    // the coefficients of bwd_apply, from the same sums
-    const float is = invstd[c], db = a, dw = b * is, invM = 1.f / (float)M;
-    const float A = weight[c] * is;
-    s_A[fin.cl] = A;
-    s_D[fin.cl] = -A * is * (dw * invM);
-    s_E[fin.cl] = -A * (db * invM);
-    if (blockIdx.x == 0) {
-      dbias[c] = db;
-      dweight[c] = dw;
-    }
-  }
-  __syncthreads();
-  if (u >= units) return;
-
-  float A[kCh], D[kCh], E[kCh];
-#pragma unroll
-  for (int k = 0; k < kCh; ++k) {
-    A[k] = s_A[col * kCh + k];
-    D[k] = s_D[col * kCh + k];
-    E[k] = s_E[col * kCh + k];
-  }
+  if (!bwd_coefficients(sg, sgx, lane, col, CB, RL, u, units, M, C, invstd, weight, dweight, dbias, ws, counters, A,
+                        D, E))
+    return;
   // phase 2: streamed rows through the ring, last read first, then the held rows.  With a residual a slot carries
   // dz (read back from dres) and x, and the held rows hold dz: the mask is already applied.
   auto unit2 = [&](int k) { return i_s + (size_t)(sn - 1 - k) * ustep; };
@@ -938,6 +1072,162 @@ __global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_bwd_fused_kernel(
   ring_fill<kBwdStages>(sn, issue2);
   ring_drain<kBwdStages>(sn, issue2, [&](int k, int slot) { apply(ring + slot * L.slot, unit2(k)); });
   for (int k = 0; k < hn; ++k) apply(hst + (size_t)k * L.step, i_h + k * ustep);
+}
+
+// The pooled backward (ReLU, no residual), in the chunking and row order of bn_act_bwd_fused_kernel.  The gradient
+// reaching row (n, h, w) of y is
+//   dyi = round(sum of g over the 1, 2 or 4 windows covering the row whose code names its position, in ascending
+//               (oh, ow) order, in fp32 from 0),   g = round(g1 + g2) of the window (g1 when g2 is nullptr),
+// which is what torch's add of the two pooled gradients, its NHWC max-pool backward and the ReLU mask give: a window
+// whose maximum carries no gradient is dead, and so is every window naming a row the ReLU zeroed.  Phase 1 forms dyi
+// from the pooled tensors (a quarter of the rows, mostly in L2) and keeps dyi and x of the held rows in shared memory;
+// phase 2 forms dyi again for the streamed rows, whose x comes through the ring.
+template <class U>
+__global__ void __launch_bounds__(kT, kResBlocksPerSM) bn_act_bwd_pool_kernel(
+    const void* __restrict__ g1, const void* __restrict__ g2, const uint32_t* __restrict__ pool_code,
+    const void* __restrict__ x, size_t M, int C, int shift, size_t rpc, int held, int H, int W, const float* mean,
+    const float* invstd, const float* weight, float* dweight, float* dbias, void* dx, float* ws, uint32_t* counters) {
+  extern __shared__ Vec16 hold[];
+  constexpr int V = Unit<U>::kVecs, SV = kT * V;
+  constexpr Layout L = fused_layout(true, false, V, true);
+  static_assert(L.step == 2 * SV && L.slot == SV, "held step: dyi, x; ring slot: x");
+  const int units = C / kCh, CB = 1 << shift, RL = kT >> shift;
+  const int col = threadIdx.x & (CB - 1), lane = threadIdx.x >> shift;
+  const int u = blockIdx.y * CB + col;
+  const size_t r0 = (size_t)blockIdx.x * rpc, r1 = min(M, r0 + rpc);
+  const int rows = (int)(r1 - r0), nh = min(held, rows);
+  const int hn = lane < nh ? (nh - 1 - lane) / RL + 1 : 0;
+  const int sn = lane < rows - nh ? (rows - nh - 1 - lane) / RL + 1 : 0;
+  Vec16* hst = hold + threadIdx.x * V;                                   // held step k at hst + k * L.step
+  Vec16* ring = hold + (size_t)(held / RL) * L.step + threadIdx.x * V;   // ring slot j at ring + j * L.slot
+  const PoolShape ps(H, W);
+  // dyi of row (n, h, w), unit u.  The covering windows are among (h / 2 + a, w / 2 + b), a, b in {0, 1}, taken in
+  // that (ascending) order; their codes are loaded together, then the gradients of the windows that name the row.
+  const size_t jrow = (size_t)ps.OW * units;
+  auto grad = [&](size_t r, float* d) {
+    size_t n;
+    int h, w;
+    ps.split(r, &n, &h, &w);
+    const int oh = h >> 1, ow = w >> 1;
+    const bool h2 = (h & 1) && oh + 1 < ps.OH, w2 = (w & 1) && ow + 1 < ps.OW;
+    const size_t j0 = (n * ps.ohw + (size_t)oh * ps.OW + ow) * units + u;
+    uint32_t cw[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const bool ok = (q & 2 ? h2 : true) && (q & 1 ? w2 : true);
+      cw[q] = ok ? __ldg(pool_code + j0 + (q & 2 ? jrow : 0) + (q & 1 ? units : 0)) : 0xffffffffu;
+    }
+    uint32_t hit[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const uint32_t pos = (uint32_t)((h - 2 * (oh + (q >> 1)) + 1) * 3 + (w - 2 * (ow + (q & 1)) + 1));
+      hit[q] = 0;
+#pragma unroll
+      for (int k = 0; k < kCh; ++k) hit[q] |= (((cw[q] >> (4 * k)) & 0xfu) == pos ? 1u : 0u) << k;
+    }
+#pragma unroll
+    for (int k = 0; k < kCh; ++k) d[k] = 0.f;
+    constexpr int QB = V == 1 ? 4 : 2;   // windows whose gradient loads are in flight together
+#pragma unroll
+    for (int q0 = 0; q0 < 4; q0 += QB) {
+      Vec16 a[QB][V], b[QB][V];
+#pragma unroll
+      for (int q = q0; q < q0 + QB; ++q) {
+        if (hit[q] == 0) continue;
+        const size_t j = j0 + (q & 2 ? jrow : 0) + (q & 1 ? units : 0);
+        const uint4* p1 = reinterpret_cast<const uint4*>(g1) + j * V;
+        const uint4* p2 = reinterpret_cast<const uint4*>(g2) + j * V;
+#pragma unroll
+        for (int v = 0; v < V; ++v) {
+          const uint4 t = __ldg(p1 + v);
+          a[q - q0][v] = Vec16{t.x, t.y, t.z, t.w};
+          if (g2 != nullptr) {
+            const uint4 e = __ldg(p2 + v);
+            b[q - q0][v] = Vec16{e.x, e.y, e.z, e.w};
+          }
+        }
+      }
+#pragma unroll
+      for (int q = q0; q < q0 + QB; ++q) {
+        if (hit[q] == 0) continue;
+        float g[kCh];
+#pragma unroll
+        for (int v = 0; v < V; ++v) U::unpack(a[q - q0][v], g + v * U::kPerVec);
+        if (g2 != nullptr) {
+          float e[kCh];
+#pragma unroll
+          for (int v = 0; v < V; ++v) U::unpack(b[q - q0][v], e + v * U::kPerVec);
+#pragma unroll
+          for (int k = 0; k < kCh; ++k) g[k] += e[k];
+          Unit<U>::round(g);   // torch's add at the junction
+        }
+#pragma unroll
+        for (int k = 0; k < kCh; ++k)
+          if ((hit[q] >> k) & 1u) d[k] += g[k];
+      }
+    }
+    Unit<U>::round(d);
+  };
+
+  // phase 1: the thread's rows in row order, x of the held ones copied to shared memory, their dyi stored beside it
+  float sg[kCh], sgx[kCh], mu[kCh];
+#pragma unroll
+  for (int k = 0; k < kCh; ++k) sg[k] = sgx[k] = 0.f;
+  auto push = [&](const float* d, const float* f) {
+#pragma unroll
+    for (int k = 0; k < kCh; ++k) {
+      sg[k] += d[k];
+      sgx[k] = fmaf(d[k], f[k] - mu[k], sgx[k]);
+    }
+  };
+  const size_t row_h = r0 + lane, row_s = r0 + nh + lane;   // the thread's first held and first streamed row
+  if (u < units) {
+#pragma unroll
+    for (int k = 0; k < kCh; ++k) mu[k] = mean[u * kCh + k];
+    for (int k = 0; k < hn; ++k) hold_copy<U>(hst + (size_t)k * L.step + SV, x, (row_h + (size_t)k * RL) * units + u);
+    cp_async_commit();
+    auto issue = [&](int k, int slot) { hold_copy<U>(ring + slot * L.slot, x, (row_s + (size_t)k * RL) * units + u); };
+    ring_fill<kBwdStages>(sn, issue);
+    cp_async_wait<kBwdStages>();
+    for (int k = 0; k < hn; ++k) {
+      Vec16* p = hst + (size_t)k * L.step;
+      float d[kCh], f[kCh];
+      grad(row_h + (size_t)k * RL, d);
+      hold_load<U>(p + SV, f);
+      push(d, f);
+#pragma unroll
+      for (int v = 0; v < V; ++v) sts16(p + v, U::pack(d + v * U::kPerVec));
+    }
+    ring_drain<kBwdStages>(sn, issue, [&](int k, int slot) {
+      float d[kCh], f[kCh];
+      grad(row_s + (size_t)k * RL, d);
+      hold_load<U>(ring + slot * L.slot, f);
+      push(d, f);
+    });
+  }
+  float A[kCh], D[kCh], E[kCh];
+  if (!bwd_coefficients(sg, sgx, lane, col, CB, RL, u, units, M, C, invstd, weight, dweight, dbias, ws, counters, A,
+                        D, E))
+    return;
+
+  // phase 2: streamed rows through the ring, last read first, then the held rows
+  auto row2 = [&](int k) { return row_s + (size_t)(sn - 1 - k) * RL; };
+  auto issue2 = [&](int k, int slot) { hold_copy<U>(ring + slot * L.slot, x, row2(k) * units + u); };
+  ring_fill<kBwdStages>(sn, issue2);
+  ring_drain<kBwdStages>(sn, issue2, [&](int k, int slot) {
+    const size_t r = row2(k);
+    float d[kCh], f[kCh];
+    grad(r, d);
+    hold_load<U>(ring + slot * L.slot, f);
+    bwd_row<U, false, false>(r * units + u, mu, A, D, E, dx, nullptr, d, f, 0u);
+  });
+  for (int k = 0; k < hn; ++k) {
+    Vec16* p = hst + (size_t)k * L.step;
+    float d[kCh], f[kCh];
+    hold_load<U>(p, d);
+    hold_load<U>(p + SV, f);
+    bwd_row<U, false, false>((row_h + (size_t)k * RL) * units + u, mu, A, D, E, dx, nullptr, d, f, 0u);
+  }
 }
 
 // ---- synchronised batch norm: the cross-rank step between the local reduction and the apply pass -------------
@@ -1057,15 +1347,19 @@ constexpr int kMaxDevices = 64;
 int dtype_index(int dtype) { return dtype == WIRE_F32 ? 0 : dtype == WIRE_BF16 ? 1 : dtype == WIRE_F16 ? 2 : -1; }
 
 using FusedFwd = void (*)(const void*, const void*, size_t, int, int, size_t, int, float, float, float*, float*,
-                          float*, float*, const float*, const float*, void*, uint8_t*, float*, uint32_t*);
+                          float*, float*, const float*, const float*, void*, uint8_t*, float*, uint32_t*, int, int,
+                          uint32_t*);
 using FusedBwd = void (*)(const void*, const void*, const void*, const uint8_t*, size_t, int, int, size_t, int,
                           const float*, const float*, const float*, float*, float*, void*, void*, float*, uint32_t*);
+using FusedBwdPool = void (*)(const void*, const void*, const uint32_t*, const void*, size_t, int, int, size_t, int,
+                              int, int, const float*, const float*, const float*, float*, float*, void*, float*,
+                              uint32_t*);
 
-// Per device: the SM count and, per direction and dtype, the dynamic shared memory a block may hold when
-// kResBlocksPerSM blocks share an SM (0: the single-launch pass cannot run on this device).
+// Per device: the SM count and, per pass (forward, backward, pooled backward) and dtype, the dynamic shared memory a
+// block may hold when kResBlocksPerSM blocks share an SM (0: the single-launch pass cannot run on this device).
 struct FusedDev {
   int sms = 0;
-  size_t dyn[2][3] = {};
+  size_t dyn[3][3] = {};
 };
 
 // Opts every variant of (direction, dtype) in to `*dyn` bytes of dynamic shared memory, first lowering *dyn by the
@@ -1092,13 +1386,18 @@ void opt_in(const K* kernels, int n, size_t share, size_t* dyn) {
 }
 
 template <class U>
-void opt_in_u(size_t share, size_t* fwd, size_t* bwd) {
-  const FusedFwd f[4] = {bn_act_fwd_fused_kernel<U, false, false>, bn_act_fwd_fused_kernel<U, false, true>,
-                         bn_act_fwd_fused_kernel<U, true, false>, bn_act_fwd_fused_kernel<U, true, true>};
+void opt_in_u(size_t share, size_t* fwd, size_t* bwd, size_t* bwd_pool) {
+  const FusedFwd f[5] = {bn_act_fwd_fused_kernel<U, false, false, false>,
+                         bn_act_fwd_fused_kernel<U, false, true, false>,
+                         bn_act_fwd_fused_kernel<U, true, false, false>,
+                         bn_act_fwd_fused_kernel<U, true, true, false>,
+                         bn_act_fwd_fused_kernel<U, true, false, true>};   // the pooled forward
   const FusedBwd b[4] = {bn_act_bwd_fused_kernel<U, false, false>, bn_act_bwd_fused_kernel<U, false, true>,
                             bn_act_bwd_fused_kernel<U, true, false>, bn_act_bwd_fused_kernel<U, true, true>};
-  opt_in(f, 4, share, fwd);
+  const FusedBwdPool bp[1] = {bn_act_bwd_pool_kernel<U>};
+  opt_in(f, 5, share, fwd);
   opt_in(b, 4, share, bwd);
+  opt_in(bp, 1, share, bwd_pool);
 }
 
 const FusedDev* fused_dev() {
@@ -1118,9 +1417,9 @@ const FusedDev* fused_dev() {
         cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev) != cudaSuccess)
       return &d;
     const size_t share = (size_t)per_sm / kResBlocksPerSM - (size_t)reserved;
-    opt_in_u<TagF32>(share, &d.dyn[0][0], &d.dyn[1][0]);
-    opt_in_u<TagBF16>(share, &d.dyn[0][1], &d.dyn[1][1]);
-    opt_in_u<TagF16>(share, &d.dyn[0][2], &d.dyn[1][2]);
+    opt_in_u<TagF32>(share, &d.dyn[0][0], &d.dyn[1][0], &d.dyn[2][0]);
+    opt_in_u<TagBF16>(share, &d.dyn[0][1], &d.dyn[1][1], &d.dyn[2][1]);
+    opt_in_u<TagF16>(share, &d.dyn[0][2], &d.dyn[1][2], &d.dyn[2][2]);
     d.sms = sms;
   }
   return &d;
@@ -1137,19 +1436,21 @@ struct FusedPlan {
 
 // The whole chunk is held when it fits (with the ring the layout always needs); otherwise the ring of kFwdStages /
 // kBwdStages row-steps comes first and the held rows get what is left (at most `cap` bytes of them when cap >= 0).
-// res selects the backward's residual layout (fused_layout).
-bool fused_plan(int bwd, int dtype, size_t M, int C, long long cap, bool res, FusedPlan* p) {
+// res selects the backward's residual layout, pool the pooled backward's (fused_layout).  The chunking depends on
+// neither, so the pooled kernels reduce in the same order as the others at the same (M, C).
+bool fused_plan(int bwd, int dtype, size_t M, int C, long long cap, bool res, FusedPlan* p, bool pool = false) {
   const int dt = dtype_index(dtype);
   const FusedDev* d = fused_dev();
-  if (dt < 0 || bad_shape(M, C) || d == nullptr || d->dyn[bwd ? 1 : 0][dt] == 0) return false;
+  const int pass = bwd ? (pool ? 2 : 1) : 0;
+  if (dt < 0 || bad_shape(M, C) || d == nullptr || d->dyn[pass][dt] == 0) return false;
   const Geo g = geo(C, red_cb(C));
   const int blocks = d->sms * kResBlocksPerSM;
   if (g.ncb > blocks) return false;
   const size_t want = (size_t)(blocks / g.ncb), rl = (size_t)g.rl;
   size_t rpc = (M + want - 1) / want;
   rpc = (rpc < rl ? rl : (rpc + rl - 1) / rl * rl);
-  const Layout L = fused_layout(bwd != 0, bwd && res, dtype == WIRE_F32 ? 2 : 1);
-  const size_t dyn = d->dyn[bwd ? 1 : 0][dt], capb = cap >= 0 ? (size_t)cap : dyn;
+  const Layout L = fused_layout(bwd != 0, bwd && res, dtype == WIRE_F32 ? 2 : 1, bwd && pool);
+  const size_t dyn = d->dyn[pass][dt], capb = cap >= 0 ? (size_t)cap : dyn;
   const size_t step = 16 * (size_t)L.step, stages = bwd ? kBwdStages : kFwdStages;   // bytes of a held row-step
   size_t held = rpc;
   int depth = 0;
@@ -1176,6 +1477,37 @@ size_t fused_bytes(const FusedPlan& p, int bwd, int dtype, size_t M, int C, bool
   const size_t e = (size_t)C * (dtype == WIRE_F32 ? 4 : 2), m = relu ? (size_t)C / kCh : 0;   // per row
   if (bwd) return M * (3 * e + m) + (res ? M * e : 0) + (dy2 ? M * e : 0) + (M - held) * (res ? 2 * e : 2 * e + m);
   return M * (2 * e + m) + (res ? M * e : 0) + (M - held) * e;
+}
+
+// The same for the pooled passes over N images of H x W (M = N H W rows, P pooled rows of C channels; the pooled
+// gradients g1 (and g2) and the codes, 4 bits a channel, are the pooled tensors).  Forward: x once, then in phase 2
+// every row a block's windows span that it does not hold (its streamed rows and the halo rows of the neighbouring
+// chunks), the pooled output and the codes written.  Backward: x and the pooled tensors once in phase 1, then x of
+// the streamed rows and the pooled tensors again for them in phase 2 (counted as that share of the pooled tensors),
+// dx written.  Re-reads of a row or pooled row within one phase of one block (the overlapping windows) are not counted.
+size_t pool_bytes(const FusedPlan& p, int bwd, int dtype, size_t M, int C, int H, int W, bool dy2) {
+  const PoolShape ps(H, W);
+  const size_t e = (size_t)C * (dtype == WIRE_F32 ? 4 : 2), P = M / ps.hw * ps.ohw, pc = (size_t)C / 2;
+  size_t held = 0, span = 0;
+  for (int g = 0; g < p.G; ++g) {
+    const size_t r0 = (size_t)g * p.rpc, r1 = r0 + p.rpc < M ? r0 + p.rpc : M;
+    const size_t h = (size_t)p.held < r1 - r0 ? (size_t)p.held : r1 - r0;
+    held += h;
+    const size_t p0 = ps.pooled_before(r0), p1 = ps.pooled_before(r1);
+    if (p0 == p1) continue;
+    size_t n;
+    int oh, ow;
+    ps.pooled_at(p0, &n, &oh, &ow);
+    const size_t c0 = n * ps.hw + (size_t)(2 * oh) * W + 2 * ow;
+    ps.pooled_at(p1 - 1, &n, &oh, &ow);
+    const size_t c1 = n * ps.hw + (size_t)(2 * oh) * W + 2 * ow;
+    const size_t lo = c0 > (size_t)W + 1 ? c0 - W - 1 : 0, hi = c1 + W + 2 < M ? c1 + W + 2 : M;
+    const size_t a = lo > r0 ? lo : r0, b = hi < r0 + h ? hi : r0 + h;   // held rows inside the span
+    span += (hi - lo) - (b > a ? b - a : 0);
+  }
+  if (!bwd) return M * e + span * e + P * (e + pc);
+  const size_t pooled = P * ((dy2 ? 2 : 1) * e + pc);
+  return 2 * M * e + pooled + (M - held) * e + (size_t)((double)pooled * (double)(M - held) / (double)M);
 }
 
 template <class... P, class... A>
@@ -1277,11 +1609,14 @@ cudaError_t launch_bn_act_fwd_stats_local(const void* x, int dtype, size_t M, in
 }
 
 bool bn_act_fused_plan(int bwd, int dtype, size_t M, int C, long long cap, int relu, int residual, int dy2,
-                       BnFusedPlan* out) {
+                       BnFusedPlan* out, int pool_h, int pool_w) {
+  const bool pool = pool_h > 0 || pool_w > 0;
+  if (pool && (pool_h < 1 || pool_w < 1 || M % ((size_t)pool_h * pool_w) != 0 || !relu || residual)) return false;
   FusedPlan p;
-  if (!fused_plan(bwd, dtype, M, C, cap, residual != 0, &p)) return false;
+  if (!fused_plan(bwd, dtype, M, C, cap, residual != 0, &p, pool)) return false;
   *out = BnFusedPlan{2 * (size_t)p.G * (size_t)C, p.g.ncb, p.rpc, p.held, p.held_bytes, p.depth, p.smem,
-                     fused_bytes(p, bwd, dtype, M, C, relu != 0, residual != 0, bwd && residual && dy2),
+                     pool ? pool_bytes(p, bwd, dtype, M, C, pool_h, pool_w, bwd && dy2)
+                          : fused_bytes(p, bwd, dtype, M, C, relu != 0, residual != 0, bwd && residual && dy2),
                      fused_dev()->sms * kResBlocksPerSM};
   return true;
 }
@@ -1297,9 +1632,44 @@ cudaError_t launch_bn_act_fwd(const void* x, const void* residual, int dtype, si
   if (!fused_plan(0, dtype, M, C, cap, residual != nullptr, &p)) return cudaErrorNotSupported;
   cudaError_t e = cudaSuccess;
   BN_DISPATCH_U(dtype, BN_DISPATCH_B(relu, kRelu, BN_DISPATCH_B(residual != nullptr, kRes, (
-      e = launch_coop(bn_act_fwd_fused_kernel<U, kRelu, kRes>, p, s, x, residual, M, C, p.g.shift, p.rpc, p.held,
-                         eps, momentum, running_mean, running_var, save_mean, save_invstd, weight, bias, y, mask, ws,
-                         counters)))));
+      e = launch_coop(bn_act_fwd_fused_kernel<U, kRelu, kRes, false>, p, s, x, residual, M, C, p.g.shift, p.rpc,
+                      p.held, eps, momentum, running_mean, running_var, save_mean, save_invstd, weight, bias, y, mask,
+                      ws, counters, 0, 0, (uint32_t*)nullptr)))));
+  return e;
+}
+
+cudaError_t launch_bn_act_fwd_pool(const void* x, int dtype, int N, int H, int W, int C, float eps, float momentum,
+                                   float* running_mean, float* running_var, float* save_mean, float* save_invstd,
+                                   const float* weight, const float* bias, void* pooled, uint32_t* code, float* ws,
+                                   uint32_t* counters, long long cap, cudaStream_t s) {
+  FusedPlan p;
+  const size_t M = (size_t)N * H * W;
+  if (N < 1 || H < 1 || W < 1 || bad_shape(M, C) || M < 2 || !aligned16(x) || !aligned16(pooled) ||
+      pooled == nullptr || code == nullptr || (running_mean == nullptr) != (running_var == nullptr))
+    return cudaErrorInvalidValue;
+  if (!fused_plan(0, dtype, M, C, cap, false, &p)) return cudaErrorNotSupported;
+  cudaError_t e = cudaSuccess;
+  BN_DISPATCH_U(dtype, (
+      e = launch_coop(bn_act_fwd_fused_kernel<U, true, false, true>, p, s, x, (const void*)nullptr, M, C, p.g.shift,
+                      p.rpc, p.held, eps, momentum, running_mean, running_var, save_mean, save_invstd, weight, bias,
+                      pooled, (uint8_t*)nullptr, ws, counters, H, W, code)));
+  return e;
+}
+
+cudaError_t launch_bn_act_bwd_pool(const void* g1, const void* g2, const uint32_t* code, const void* x, int dtype,
+                                   int N, int H, int W, int C, const float* mean, const float* invstd,
+                                   const float* weight, float* dweight, float* dbias, void* dx, float* ws,
+                                   uint32_t* counters, long long cap, cudaStream_t s) {
+  FusedPlan p;
+  const size_t M = (size_t)N * H * W;
+  if (N < 1 || H < 1 || W < 1 || bad_shape(M, C) || g1 == nullptr || code == nullptr || !aligned16(g1) ||
+      !aligned16(g2) || !aligned16(x) || !aligned16(dx))
+    return cudaErrorInvalidValue;
+  if (!fused_plan(1, dtype, M, C, cap, false, &p, true)) return cudaErrorNotSupported;
+  cudaError_t e = cudaSuccess;
+  BN_DISPATCH_U(dtype, (
+      e = launch_coop(bn_act_bwd_pool_kernel<U>, p, s, g1, g2, code, x, M, C, p.g.shift, p.rpc, p.held, H, W, mean,
+                      invstd, weight, dweight, dbias, dx, ws, counters)));
   return e;
 }
 

@@ -71,8 +71,10 @@ struct BnFusedPlan {
   int wave_blocks;         // blocks in one wave on this device: the grid is at most this large
 };
 // residual selects the backward's layout too (a residual backward needs more shared memory per ring slot).
+// pool_h, pool_w > 0: the pooled passes below over images of pool_h x pool_w (M a multiple of pool_h * pool_w; relu
+// and no residual), whose bytes_moved counts the pooled tensors, the halo rows and their re-reads.
 bool bn_act_fused_plan(int bwd, int dtype, size_t M, int C, long long cap, int relu, int residual, int dy2,
-                       BnFusedPlan* plan);
+                       BnFusedPlan* plan, int pool_h = 0, int pool_w = 0);
 cudaError_t launch_bn_act_fwd(const void* x, const void* residual, int dtype, size_t M, int C, float eps,
                               float momentum, float* running_mean, float* running_var, float* save_mean,
                               float* save_invstd, const float* weight, const float* bias, int relu, void* y,
@@ -82,6 +84,25 @@ cudaError_t launch_bn_act_bwd(const void* dy, const void* dy2, const void* x, co
                               int C, const float* mean, const float* invstd, const float* weight, float* dweight,
                               float* dbias, void* dx, void* dresidual, float* ws, uint32_t* counters, long long cap,
                               cudaStream_t s);
+
+// ---- pooled single-launch passes: ReLU, then a max pool of kernel 3, stride 2, padding 1 (ResNet's stem) -------
+//
+// Over N NHWC images of H x W x C; the pooled output is N x OH x OW x C with OH = (H - 1) / 2 + 1 and likewise OW.
+//   fwd_pool   launch_bn_act_fwd's statistics, bit for bit; writes the pooled output (what torch's max_pool2d of y
+//              gives) and, per pooled row and 8 channels, one uint32 of 4-bit window codes (N * OH * OW * C / 8
+//              words) instead of y and the mask
+//   bwd_pool   for the gradients g1 and g2 (nullptr: none) of the pooled output: dx, dweight and dbias of
+//              launch_bn_act_bwd fed what torch's add of g1 and g2, max-pool backward and ReLU mask produce, bit for
+//              bit, without that gradient ever being stored
+// Plans, workspaces and cap as for the single-launch passes (bn_act_fused_plan with pool_h = H, pool_w = W).
+cudaError_t launch_bn_act_fwd_pool(const void* x, int dtype, int N, int H, int W, int C, float eps, float momentum,
+                                   float* running_mean, float* running_var, float* save_mean, float* save_invstd,
+                                   const float* weight, const float* bias, void* pooled, uint32_t* code, float* ws,
+                                   uint32_t* counters, long long cap, cudaStream_t s);
+cudaError_t launch_bn_act_bwd_pool(const void* g1, const void* g2, const uint32_t* code, const void* x, int dtype,
+                                   int N, int H, int W, int C, const float* mean, const float* invstd,
+                                   const float* weight, float* dweight, float* dbias, void* dx, float* ws,
+                                   uint32_t* counters, long long cap, cudaStream_t s);
 
 // ---- synchronised batch norm (torch.nn.SyncBatchNorm semantics) over peer-mapped memory --------------------
 //

@@ -4,7 +4,9 @@ reference's headline synthetic benchmark.
 A block's output feeds two consumers in the next block: conv1 and the skip path (the identity residual or the
 downsample).  Inside ResNet.forward the blocks pass a ``(main, skip)`` pair, the last batch norm of a block returning
 its output and an alias of it, so the two gradients reach that batch norm's backward separately and its kernel sums
-them as it reads them (ops/bn_act.py).  A block called on one tensor uses it for both and returns one tensor."""
+them as it reads them (ops/bn_act.py).  The stem's batch norm does the same for the max-pooled output that feeds
+layer1, and runs the ReLU and the max pool in its own kernels.  A block called on one tensor uses it for both and
+returns one tensor."""
 import torch
 import torch.nn as nn
 
@@ -95,8 +97,8 @@ class ResNet(nn.Module):
         return nn.Sequential(*layers)
 
     def forward(self, x):
-        x = self.maxpool(self.bn1(self.conv1(x)))
-        x, _ = self.layer4(self.layer3(self.layer2(self.layer1((x, x)))))   # the max pool's junction: autograd sums
+        x = self.bn1(self.conv1(x), pool=self.maxpool, pair=True)   # the stem's batch norm, ReLU and max pool
+        x, _ = self.layer4(self.layer3(self.layer2(self.layer1(x))))
         return self.fc(torch.flatten(self.avgpool(x), 1))
 
 

@@ -11,6 +11,10 @@ and threshold-backward passes.  Every other input - CPU, eval mode, NCHW, C not 
 ``forward(x, residual, pair=True)`` returns ``(y, alias of y)`` for an output with two consumers (a ResNet block's
 output feeds the next block's conv1 and its skip path).  Autograd then hands backward the two gradients separately,
 and the single-launch backward sums them as it reads them instead of a separate ``add`` pass over the tensor.
+
+``forward(x, pool=nn.MaxPool2d(3, 2, 1), pair=True)`` returns ``pool`` of the output (and an alias of it): ResNet's
+stem.  With ReLU on a fusable input the pooled kernels compute it in one launch per direction, without storing y, its
+mask or the pool's indices; otherwise it is ``pool`` of the unpooled path.
 """
 from __future__ import annotations
 
@@ -128,6 +132,83 @@ class _BatchNormActFn(torch.autograd.Function):
         return dx, dres, dweight, dbias, None, None, None, None, None, None
 
 
+def _stem_pool(pool) -> bool:
+    """Whether ``pool`` is the max pool the pooled kernels implement: kernel 3, stride 2, padding 1, dilation 1, no
+    ceil mode, no indices returned (ResNet's stem)."""
+    two = lambda v: tuple(v) if isinstance(v, (tuple, list)) else (v, v)  # noqa: E731
+    return (isinstance(pool, nn.MaxPool2d) and two(pool.kernel_size) == (3, 3) and two(pool.stride) == (2, 2)
+            and two(pool.padding) == (1, 1) and two(pool.dilation) == (1, 1) and not pool.ceil_mode
+            and not pool.return_indices)
+
+
+def _pool_planned(x) -> bool:
+    """Whether the pooled forward and backward can both run at x's shape on its device."""
+    cu = _native.cuda()
+    n, c, h, w = x.shape
+    code, m = _CODES[x.dtype], n * h * w
+    return all(cu.bn_act_plan(d, code, m, c, _cap(), relu=True, pool_h=h, pool_w=w) is not None for d in (0, 1))
+
+
+def _pooled_grad(g, x):
+    """A pooled gradient as the kernel reads it: x's dtype, channels_last, 16-byte aligned."""
+    g = g.to(x.dtype).contiguous(memory_format=torch.channels_last)
+    return g if g.data_ptr() % 16 == 0 else g.clone(memory_format=torch.channels_last)
+
+
+class _BatchNormActPoolFn(torch.autograd.Function):
+    """Batch norm, ReLU and the stem's max pool (``_stem_pool``) as one single-launch kernel per direction.
+
+    Forward writes the pooled output and a 4-bit window code per channel instead of y and its ReLU mask.  With
+    ``pair`` the output is ``(p, p.view_as(p))`` and backward receives the two pooled gradients separately (None for
+    an alias nobody used); the kernel sums them as torch's add would while it forms the max-pool and ReLU backward,
+    so the gradient at y is never stored.  The caller checks both plans (``_pool_planned``) first."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, running_mean, running_var, momentum, eps, pair):
+        cu = _native.cuda()
+        n, c, h, w = x.shape
+        code = _CODES[x.dtype]
+        stream = torch.cuda.current_stream(x.device).cuda_stream
+        f32 = dict(dtype=torch.float32, device=x.device)
+        mean, invstd = torch.empty(c, **f32), torch.empty(c, **f32)
+        oh, ow = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+        p = torch.empty((n, c, oh, ow), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
+        codes = torch.empty((n * oh * ow, c // _UNIT), dtype=torch.int32, device=x.device)
+        plan = cu.bn_act_plan(0, code, n * h * w, c, _cap(), relu=True, pool_h=h, pool_w=w)
+        ws, ctr = _workspace(plan["ws_floats"], plan["counters"], x.device)
+        cu.bn_act_fwd_pool(x.data_ptr(), code, n, h, w, c, float(eps), float(momentum), _ptr(running_mean),
+                           _ptr(running_var), mean.data_ptr(), invstd.data_ptr(), weight.data_ptr(), bias.data_ptr(),
+                           p.data_ptr(), codes.data_ptr(), ws.data_ptr(), ctr.data_ptr(), stream, _cap())
+        ctx.save_for_backward(x, weight, mean, invstd, codes)
+        if pair:
+            ctx.set_materialize_grads(False)
+            return p, p.view_as(p)
+        return p
+
+    @staticmethod
+    def backward(ctx, g1, g2=None):
+        x, weight, mean, invstd, codes = ctx.saved_tensors
+        cu = _native.cuda()
+        n, c, h, w = x.shape
+        code = _CODES[x.dtype]
+        if g1 is None:
+            g1, g2 = g2, None
+        g1 = _pooled_grad(g1, x)
+        g2 = None if g2 is None else _pooled_grad(g2, x)
+        stream = torch.cuda.current_stream(x.device).cuda_stream
+        f32 = dict(dtype=torch.float32, device=x.device)
+        dweight, dbias = torch.empty(c, **f32), torch.empty(c, **f32)
+        dx = torch.empty_like(x)
+        plan = cu.bn_act_plan(1, code, n * h * w, c, _cap(), relu=True, pool_h=h, pool_w=w)
+        if plan is None:
+            raise RuntimeError("bn_act_bwd_pool cannot run at %s on this device" % (tuple(x.shape),))
+        ws, ctr = _workspace(plan["ws_floats"], plan["counters"], x.device)
+        cu.bn_act_bwd_pool(g1.data_ptr(), _ptr(g2), codes.data_ptr(), x.data_ptr(), code, n, h, w, c,
+                           mean.data_ptr(), invstd.data_ptr(), weight.data_ptr(), dweight.data_ptr(),
+                           dbias.data_ptr(), dx.data_ptr(), ws.data_ptr(), ctr.data_ptr(), stream, _cap())
+        return dx, dweight, dbias, None, None, None, None, None
+
+
 class BatchNormAct2d(nn.BatchNorm2d):
     """``nn.BatchNorm2d`` followed by an optional residual add and activation (``act``: None or "relu")."""
 
@@ -151,9 +232,16 @@ class BatchNormAct2d(nn.BatchNorm2d):
         return _BatchNormActFn.apply(x, residual, self.weight, self.bias, running_mean, running_var, factor, self.eps,
                                      self.act == "relu", pair)
 
-    def forward(self, x, residual=None, pair=False):
-        """``act(batch_norm(x) [+ residual])``; with ``pair``, ``(y, alias of y)`` for two consumers of y (see the
-        module docstring).  Neither tensor of the pair may be modified in place."""
+    def _poolable(self, x, pool):
+        """Whether ``pool(relu(batch_norm(x)))`` can take the pooled single-launch kernels (``_fusable`` checked)."""
+        return self.act == "relu" and _stem_pool(pool) and _pool_planned(x)
+
+    def forward(self, x, residual=None, pair=False, pool=None):
+        """``act(batch_norm(x) [+ residual])``, then ``pool`` of it when one is given; with ``pair``, ``(out, alias
+        of out)`` for two consumers of the output (see the module docstring).  Neither tensor of the pair may be
+        modified in place."""
+        if pool is not None:
+            return self._forward_pooled(x, residual, pair, pool)
         # statistics bookkeeping exactly as nn.BatchNorm2d.forward
         self._check_input_dim(x)
         factor = 0.0 if self.momentum is None else self.momentum
@@ -172,6 +260,22 @@ class BatchNormAct2d(nn.BatchNorm2d):
         if self.act == "relu":
             y = F.relu(y, inplace=True)
         return (y, y) if pair else y
+
+    def _forward_pooled(self, x, residual, pair, pool):
+        """``pool`` of the output: the pooled kernels for the stem's ReLU and max pool on a fusable input without a
+        residual, ``pool`` of the unpooled path otherwise."""
+        self._check_input_dim(x)
+        batch_stats = self.training or (self.running_mean is None and self.running_var is None)
+        if residual is None and self._fusable(x, None, batch_stats) and self._poolable(x, pool):
+            factor = 0.0 if self.momentum is None else self.momentum
+            if self.training and self.track_running_stats and self.num_batches_tracked is not None:
+                self.num_batches_tracked.add_(1)
+                factor = 1.0 / float(self.num_batches_tracked) if self.momentum is None else self.momentum
+            track = not self.training or self.track_running_stats
+            return _BatchNormActPoolFn.apply(x, self.weight, self.bias, self.running_mean if track else None,
+                                             self.running_var if track else None, factor, self.eps, pair)
+        p = pool(self.forward(x, residual))
+        return (p, p) if pair else p
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -333,6 +437,9 @@ class SyncBatchNormAct2d(BatchNormAct2d):
     def _fusable(self, x, residual, batch_stats):
         return True if self._synced() else super()._fusable(x, residual, batch_stats)
 
+    def _poolable(self, x, pool):
+        return False   # no pooled synchronised kernels: pool of the synchronised (or, at world 1, plain) path
+
     def _fused(self, x, residual, running_mean, running_var, factor, pair=False):
         if not self._synced():
             return super()._fused(x, residual, running_mean, running_var, factor, pair)
@@ -340,13 +447,13 @@ class SyncBatchNormAct2d(BatchNormAct2d):
                                       self.eps, self.act == "relu", self.sync)
         return (y, y) if pair else y   # autograd sums the two gradients
 
-    def forward(self, x, residual=None, pair=False):
+    def forward(self, x, residual=None, pair=False, pool=None):
         if self._synced():
             self._check_input_dim(x)
             why = self._unfusable(x, residual)
             if why is not None:
                 raise ValueError("SyncBatchNormAct2d: synchronised training needs a fusable input, but %s" % why)
-        return super().forward(x, residual, pair)
+        return super().forward(x, residual, pair, pool)
 
 
 def convert_sync_batchnorm(module: nn.Module, sync: Optional[SyncBatchNormContext]) -> nn.Module:

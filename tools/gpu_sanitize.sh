@@ -27,7 +27,11 @@ else
        "tests/test_gpu_bn_act_junction.py::test_two_gradients_match_torch_sum[1x24x37x3-bfloat16-part]"
        "tests/test_gpu_bn_act_junction.py::test_two_gradients_match_torch_sum[64x1024x14x14-bfloat16-part]"
        "tests/test_gpu_bn_act_junction.py::test_second_gradient_fallbacks[3x8x5x7-bfloat16-misaligned]"
-       "tests/test_gpu_bn_act_junction.py::test_second_gradient_fallbacks[2x40x9x7-float32-nchw]")
+       "tests/test_gpu_bn_act_junction.py::test_second_gradient_fallbacks[2x40x9x7-float32-nchw]"
+       "tests/test_gpu_bn_act_pool.py::test_pooled_matches_stock_chain[3x8x5x7-bfloat16-full]"
+       "tests/test_gpu_bn_act_pool.py::test_pooled_matches_stock_chain[2x40x9x7-float32-part]"
+       "tests/test_gpu_bn_act_pool.py::test_pooled_matches_stock_chain[1x8x1x6-float16-none]"
+       "tests/test_gpu_bn_act_pool.py::test_pooled_matches_stock_chain[2x16x7x1-bfloat16-none]")
 fi
 timeout 1200 compute-sanitizer --tool "$TOOL" --error-exitcode 3 \
   --log-file "$OUT"/sanitizer_"$TOOL".log \
