@@ -6,7 +6,9 @@
 ReLU mask) and one backward (reduce, grid barrier, apply), or two each (the same phases as separate launches) where
 the device cannot run the single-launch kernels at that shape, instead of torch's separate batch-norm, add, ReLU
 and threshold-backward passes.  Every other input - CPU, eval mode, NCHW, C not a multiple of 8 - takes the stock
-``F.batch_norm`` / add / ``relu`` composition, which computes the same function.
+``F.batch_norm`` / add / ``relu`` composition, which computes the same function.  A channels_last view whose data
+does not start on a 16-byte boundary (x, the residual or a gradient) is copied to one that does before the kernels
+read it.
 
 ``forward(x, residual, pair=True)`` returns ``(y, alias of y)`` for an output with two consumers (a ResNet block's
 output feeds the next block's conv1 and its skip path).  Autograd then hands backward the two gradients separately,
@@ -55,6 +57,12 @@ def _sum_in_kernel(dy, dy2, x) -> bool:
             and dy2.data_ptr() % 16 == 0)
 
 
+def _aligned(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+    """t, or a channels_last copy of it when its data does not start on the 16-byte boundary the kernels' vector
+    loads need (a view at an odd element offset)."""
+    return t if t is None or t.data_ptr() % 16 == 0 else t.clone(memory_format=torch.channels_last)
+
+
 def _workspace(nws, nctr, device):
     return (torch.empty(nws, dtype=torch.float32, device=device),
             torch.zeros(nctr, dtype=torch.int32, device=device))
@@ -69,6 +77,7 @@ class _BatchNormActFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, residual, weight, bias, running_mean, running_var, momentum, eps, relu, pair=False):
         cu = _native.cuda()
+        x, residual = _aligned(x), _aligned(residual)
         n, c, h, w = x.shape
         m = n * h * w
         code = _CODES[x.dtype]
@@ -115,7 +124,7 @@ class _BatchNormActFn(torch.autograd.Function):
         plan = cu.bn_act_plan(1, code, m, c, _cap(), residual=ctx.has_residual)
         if dy2 is not None and not (plan is not None and ctx.has_residual and _sum_in_kernel(dy, dy2, x)):
             dy, dy2 = dy + dy2, None
-        dy = dy.to(x.dtype).contiguous(memory_format=torch.channels_last)
+        dy = _aligned(dy.to(x.dtype).contiguous(memory_format=torch.channels_last))
         if plan is not None:
             ws, ctr = _workspace(plan["ws_floats"], plan["counters"], x.device)
             cu.bn_act_bwd(dy.data_ptr(), x.data_ptr(), _ptr(mask), code, m, c, mean.data_ptr(), invstd.data_ptr(),
@@ -151,8 +160,7 @@ def _pool_planned(x) -> bool:
 
 def _pooled_grad(g, x):
     """A pooled gradient as the kernel reads it: x's dtype, channels_last, 16-byte aligned."""
-    g = g.to(x.dtype).contiguous(memory_format=torch.channels_last)
-    return g if g.data_ptr() % 16 == 0 else g.clone(memory_format=torch.channels_last)
+    return _aligned(g.to(x.dtype).contiguous(memory_format=torch.channels_last))
 
 
 class _BatchNormActPoolFn(torch.autograd.Function):
@@ -166,6 +174,7 @@ class _BatchNormActPoolFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, bias, running_mean, running_var, momentum, eps, pair):
         cu = _native.cuda()
+        x = _aligned(x)
         n, c, h, w = x.shape
         code = _CODES[x.dtype]
         stream = torch.cuda.current_stream(x.device).cuda_stream
@@ -342,6 +351,7 @@ class _SyncBatchNormActFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, residual, weight, bias, running_mean, running_var, momentum, eps, relu, sync):
         cu = _native.cuda()
+        x, residual = _aligned(x), _aligned(residual)
         n, c, h, w = x.shape
         m = n * h * w
         code = _CODES[x.dtype]
@@ -375,7 +385,7 @@ class _SyncBatchNormActFn(torch.autograd.Function):
         n, c, h, w = x.shape
         m = n * h * w
         code = _CODES[x.dtype]
-        dy = dy.to(x.dtype).contiguous(memory_format=torch.channels_last)
+        dy = _aligned(dy.to(x.dtype).contiguous(memory_format=torch.channels_last))
         stream = sync.stream_for(x.device)
         f32 = dict(dtype=torch.float32, device=x.device)
         dweight, dbias = torch.empty(c, **f32), torch.empty(c, **f32)

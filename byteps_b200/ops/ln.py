@@ -8,7 +8,8 @@ multiple of 8 and at most 2048, with affine parameters in fp32 or the activation
 writes the output, z = residual + dropout(y), the per-row mean and rstd and a 1-bit keep mask, and backward is one
 launch that writes d(residual), dy, dgamma and dbeta; torch runs dropout, the add and layer_norm as separate passes
 each way.  Every other input takes the stock ``F.dropout`` / add / ``F.layer_norm`` composition, which computes the
-same function.
+same function.  A tensor whose data does not start on a 16-byte boundary (a view at an odd element offset) is copied
+to one that does before the kernels read it.
 
 Dropout bits come from Philox4x32-10 keyed by a (seed, offset) pair drawn on the device from torch's CUDA generator
 on every call, so ``torch.manual_seed`` reproduces them and each replay of a captured CUDA graph draws new ones.
@@ -33,6 +34,12 @@ def _ptr(t: Optional[torch.Tensor]) -> int:
     return 0 if t is None else t.data_ptr()
 
 
+def _aligned(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+    """t, or a contiguous copy of it when its data does not start on the 16-byte boundary the kernels' vector loads
+    need (a view at an odd element offset)."""
+    return t if t is None or t.data_ptr() % 16 == 0 else t.clone(memory_format=torch.contiguous_format)
+
+
 def _keep_threshold(p: float) -> int:
     return min(int(round((1.0 - p) * 2.0 ** 32)), 2 ** 32 - 1)
 
@@ -41,6 +48,7 @@ class _DropoutAddLayerNormFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, y, residual, weight, bias, p, eps, grad):
         cu = _native.cuda()
+        y, residual, weight, bias = _aligned(y), _aligned(residual), _aligned(weight), _aligned(bias)
         h = y.shape[-1]
         m = y.numel() // h
         code, wcode = _CODES[y.dtype], _CODES[weight.dtype]
@@ -73,7 +81,7 @@ class _DropoutAddLayerNormFn(torch.autograd.Function):
         h = z.shape[-1]
         m = z.numel() // h
         code, wcode = _CODES[z.dtype], _CODES[weight.dtype]
-        dout = dout.to(z.dtype).contiguous()
+        dout = _aligned(dout.to(z.dtype).contiguous())
         stream = torch.cuda.current_stream(z.device).cuda_stream
         dweight, dbias = torch.empty_like(weight), torch.empty_like(weight)
         dres = torch.empty_like(z) if ctx.has_residual else None
