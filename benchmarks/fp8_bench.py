@@ -11,6 +11,14 @@ Per layer: M = 8192 tokens (batch 64 x sequence 128) and (K, N) = (1024, 3072) q
                (4 bytes per element moved), plus the bias
     gemm       the three FP8 GEMMs alone (_scaled_mm, no fast accumulation); 2 M N K FLOP forward, 4 M N K backward
 
+Feed-forward block (fc1 -> GELU -> fc2 of BERT-large, M = 8192, K = 1024, I = 4096, with bias):
+
+    mlp        composed fc2(F.gelu(fc1(x))) of two Fp8Linear, and fused ops.fp8.fp8_gelu_mlp: forward, and forward +
+               backward with every gradient
+    actcast    the fused casts alone at [M, I]: ACT_GELU z -> E4M3 rows + transposed (read z, write two FP8 copies:
+               4 bytes per element) and ACT_DGELU (dh, z) -> E5M2 rows + transposed + the bias gradient (read dh
+               and z, write two copies: 6 bytes per element, plus the bias)
+
 Each timed call runs on the next of enough copies of its inputs that they span more than --rotate-mb, so no call finds
 its input in the 50 MB L2; --iters calls are captured in one CUDA graph and its replays are timed with CUDA events.
 Shares of peak are against the H100 SXM data sheet (3.35 TB/s; 1979 dense FP8 TFLOP/s and 989 bf16 TFLOP/s), figures
@@ -21,10 +29,12 @@ DistributedOptimizer(fused_update=True), the whole step captured in one CUDA gra
 the bf16 graph is captured first, then the encoder's qkv / proj / fc1 / fc2 become Fp8Linear (the same parameters, as
 bert_large(fp8_linear=True) builds them) and the fp8 graph is captured; the two graphs are timed alternately,
 --rounds rounds of --steps replays each.  Memory is the peak allocated while each graph is warmed up and captured,
-above what was allocated before.  The GPU name, power limit and SM clock are read in the same run.
+above what was allocated before.  The GPU name, power limit and SM clock are read in the same run.  Then, the
+same way, BERT-large with fp8_linear=True, fused_norm=True and fused_loss=True twice: its encoder MLPs through the
+composition fc2(F.gelu(fc1(x))) and through fp8_gelu_mlp (the model as it ships), two graphs timed alternately.
 
     python benchmarks/fp8_bench.py [--iters 20] [--reps 5] [--rotate-mb 600] [--steps 20] [--rounds 5] [--no-step]
-                                   [--json f]
+                                   [--only-mlp] [--json f]
 """
 import argparse
 import json
@@ -58,6 +68,26 @@ def cast_bytes(kind, k, n):
     return 4 * M * n + 2 * n
 
 
+def _graphed_us(args, torch, fn, k):
+    for i in range(k):
+        fn(i)
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        for i in range(args.iters):
+            fn(i % k)
+    g.replay()
+    torch.cuda.synchronize()
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    for _ in range(args.reps):
+        g.replay()
+    b.record()
+    torch.cuda.synchronize()
+    del g
+    return a.elapsed_time(b) * 1e3 / (args.reps * args.iters)
+
+
 def per_layer(args, torch, rows):
     import torch.nn as nn
 
@@ -68,23 +98,7 @@ def per_layer(args, torch, rows):
     dt = torch.bfloat16
 
     def graphed_us(fn, k):
-        for i in range(k):
-            fn(i)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            for i in range(args.iters):
-                fn(i % k)
-        g.replay()
-        torch.cuda.synchronize()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        for _ in range(args.reps):
-            g.replay()
-        b.record()
-        torch.cuda.synchronize()
-        del g
-        return a.elapsed_time(b) * 1e3 / (args.reps * args.iters)
+        return _graphed_us(args, torch, fn, k)
 
     def row(layer, k, n, path, kind, us, nbytes=None, flop=None):
         r = dict(layer=layer, K=k, N=n, path=path, kind=kind, us=us)
@@ -159,6 +173,134 @@ def per_layer(args, torch, rows):
         row(name, k, n, "gemm", "fwd", graphed_us(gemm_fwd, copies), flop=flop)
         row(name, k, n, "gemm", "bwd", graphed_us(gemm_bwd, copies), flop=2 * flop)
         del X, DYs, ops
+
+
+def per_block(args, torch, rows):
+    """fc1 -> GELU -> fc2 composed and fused, and the two fused casts alone"""
+    import copy
+
+    import torch.nn.functional as F
+
+    from byteps_b200.ops import fp8
+    from byteps_b200.ops.fp8 import Fp8Linear, fp8_gelu_mlp
+
+    dev = torch.device("cuda", 0)
+    dt = torch.bfloat16
+    k, i = 1024, 4096
+    gen = torch.Generator(device=dev).manual_seed(0)
+    copies = max(2, int(-(-args.rotate_mb * 1e6 // (2 * M * i))))
+    X = [torch.randn(M, k, device=dev, generator=gen, dtype=dt).requires_grad_(True) for _ in range(copies)]
+    DY = [torch.randn(M, k, device=dev, generator=gen, dtype=dt) for _ in range(copies)]
+    torch.manual_seed(0)
+    fc1, fc2 = Fp8Linear(k, i).to(dev).to(dt), Fp8Linear(i, k).to(dev).to(dt)
+    mods = {"composed": (copy.deepcopy(fc1), copy.deepcopy(fc2)), "fused": (fc1, fc2)}
+    paths = {"composed": lambda x, m1, m2: m2(F.gelu(m1(x))), "fused": fp8_gelu_mlp}
+    res = {}
+    for path in ("composed", "fused"):
+        m1, m2 = mods[path]
+        f = paths[path]
+        params = list(m1.parameters()) + list(m2.parameters())
+
+        def fwd(j, f=f, m1=m1, m2=m2):
+            f(X[j], m1, m2)
+
+        def both(j, f=f, m1=m1, m2=m2, params=params):
+            torch.autograd.grad(f(X[j], m1, m2), [X[j]] + params, DY[j])
+
+        res[path] = (_graphed_us(args, torch, fwd, copies), _graphed_us(args, torch, both, copies))
+    for path in ("composed", "fused"):
+        us_f, us_fb = res[path]
+        rows.append(dict(block="mlp", K=k, I=i, path=path, fwd_us=us_f, fwd_bwd_us=us_fb))
+        print("mlp   %5d %5d %-8s fwd %9.1f us   fwd+bwd %9.1f us" % (k, i, path, us_f, us_fb))
+    print("mlp   fused saves %.1f us forward and %.1f us forward + backward per layer" % (
+        res["composed"][0] - res["fused"][0], res["composed"][1] - res["fused"][1]))
+    del X, DY
+
+    Z = [torch.randn(M, i, device=dev, generator=gen, dtype=dt) for _ in range(copies)]
+    DH = [torch.randn(M, i, device=dev, generator=gen, dtype=dt) for _ in range(copies)]
+    st = fp8.ScalingState(dev)
+    fp8.seed(F.gelu(Z[0]), st.row(fp8.X), fp8.E4M3)
+    fp8.seed(torch.ops.aten.gelu_backward(DH[0], Z[0]), st.row(fp8.DY), fp8.E5M2)
+
+    def gelu_cast(j):
+        fp8.cast(Z[j], st.row(fp8.X), fp8.E4M3, fp8.BOTH, act=fp8.ACT_GELU)
+
+    def dgelu_cast(j):
+        fp8.cast(DH[j], st.row(fp8.DY), fp8.E5M2, fp8.BOTH, dt, act=fp8.ACT_DGELU, aux=Z[j])
+
+    for kind, fn, nbytes in (("gelu", gelu_cast, 4 * M * i), ("dgelu", dgelu_cast, 6 * M * i + 2 * i)):
+        us = _graphed_us(args, torch, fn, copies)
+        gbs = nbytes / (us * 1e3)
+        rows.append(dict(block="actcast", M=M, I=i, kind=kind, us=us, bytes=nbytes, gbs=gbs,
+                         peak_share=gbs / PEAK_GBS))
+        print("actcast [%d, %d] %-5s %9.1f us %8.0f GB/s %5.1f%% of 3.35 TB/s" % (M, i, kind, us, gbs,
+                                                                                 100 * gbs / PEAK_GBS))
+    del Z, DH
+
+
+def mlp_step(args, torch, rows):
+    """BERT-large fp8_linear step with the encoder MLPs composed vs fused, two graphs timed alternately"""
+    import torch.nn.functional as F
+
+    import byteps_b200.models.bert as bert
+    import byteps_b200.torch as bps
+    from byteps_b200.torch.graph import GraphedStep
+
+    dev = torch.device("cuda", 0)
+    bps.init()
+    torch.manual_seed(0)
+    model = bert.bert_large(fp8_linear=True, fused_norm=True, fused_loss=True).to(dev).to(torch.bfloat16).train()
+    opt = bps.DistributedOptimizer(torch.optim.AdamW(model.parameters(), lr=1e-4, weight_decay=0.01),
+                                   named_parameters=model.named_parameters(), fused_update=True)
+    gen = torch.Generator().manual_seed(1234)
+    ids = torch.randint(0, 30522, (args.batch, args.seq), generator=gen).to(dev)
+    labels = torch.randint(0, 30522, (args.batch, args.seq), generator=gen).to(dev)
+
+    def step():
+        opt.zero_grad()
+        loss = model(ids, mlm_labels=labels)
+        loss.backward()
+        opt.step()
+        return loss
+
+    fused_mlp = bert.fp8_gelu_mlp
+    graphs = {}
+    for name in ("composed", "fused"):
+        bert.fp8_gelu_mlp = (lambda x, fc1, fc2: fc2(F.gelu(fc1(x)))) if name == "composed" else fused_mlp
+        try:
+            graphs[name] = GraphedStep(step, warmup=3, pre_replay=opt.refresh_hparams, device=dev)
+        finally:
+            bert.fp8_gelu_mlp = fused_mlp
+
+    def timed(g):
+        for _ in range(3):
+            g()
+        torch.cuda.synchronize()
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        for _ in range(args.steps):
+            g()
+        b.record()
+        torch.cuda.synchronize()
+        return a.elapsed_time(b) / args.steps
+
+    ms = {"composed": [], "fused": []}
+    for _ in range(args.rounds):
+        for name in ("composed", "fused"):
+            ms[name].append(timed(graphs[name]))
+    info = gpu_info()
+    for name in ("composed", "fused"):
+        med = statistics.median(ms[name])
+        spread = max(ms[name]) - min(ms[name])
+        rows.append(dict(step="fp8_linear_mlp_" + name, ms=ms[name], median_ms=med, spread_ms=spread,
+                         tokens_per_s=args.batch * args.seq / (med / 1e3)))
+        print("BERT-large fp8_linear step, MLP %-8s ms per step over %d rounds: %s  (median %.2f ms, spread "
+              "%.2f ms)" % (name, args.rounds, " ".join("%.2f" % v for v in ms[name]), med, spread))
+    print("fused MLP saves %.2f ms per step (medians)" % (statistics.median(ms["composed"]) -
+                                                          statistics.median(ms["fused"])))
+    print("GPU after the step rounds: %s" % info)
+    del graphs
+    bps.shutdown()
 
 
 def whole_step(args, torch, rows):
@@ -240,6 +382,7 @@ def main():
     ap.add_argument("--steps", type=int, default=20, help="timed replays of a whole step per round")
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--no-step", action="store_true", help="per-layer table only")
+    ap.add_argument("--only-mlp", action="store_true", help="only the feed-forward block rows and its step")
     ap.add_argument("--json", default=None, help="also write the rows as JSON to this file")
     args = ap.parse_args()
 
@@ -254,9 +397,13 @@ def main():
     info = gpu_info()
     print("GPU: %s; M = %d, bf16 inputs" % (info, M))
     rows = []
-    per_layer(args, torch, rows)
+    if not args.only_mlp:
+        per_layer(args, torch, rows)
+    per_block(args, torch, rows)
     if not args.no_step:
-        whole_step(args, torch, rows)
+        if not args.only_mlp:
+            whole_step(args, torch, rows)
+        mlp_step(args, torch, rows)
     if args.json:
         with open(args.json, "w") as fh:
             json.dump({"gpu": info, "rows": rows}, fh, indent=1)

@@ -6,6 +6,10 @@
 // transposed copy it also stores them in a 16 KB shared tile whose 16-byte chunks are XOR-swizzled by row / 16; each
 // thread then reads a 16-row x 4-column patch (sixteen 32-bit words, no bank conflicts), transposes it with byte
 // permutes and writes four 16-byte rows of the [K, M] copy.  The grid is one resident wave (occupancy API).
+//
+// An optional elementwise prologue (ACT) turns each loaded value into torch's GELU of it, or into torch's GELU
+// gradient of it at the matching element of a second input, rounded to the input dtype as torch stores them; the
+// amax, the bias sums and the cast then see exactly the tensor the unfused torch op would have written.
 #include "kernels/fp8.cuh"
 
 #include <math.h>
@@ -51,6 +55,21 @@ __device__ __forceinline__ Vec16 pack16(const float* f) {
   for (int k = 0; k < 4; ++k) w[k] = F::cvt2(f[4 * k], f[4 * k + 1]) | F::cvt2(f[4 * k + 2], f[4 * k + 3]) << 16;
   return Vec16{w[0], w[1], w[2], w[3]};
 }
+
+// torch's GELU (erf form) and its gradient, in the order torch's sm_90 kernels evaluate them: every operation is
+// pinned with an _rn intrinsic so that contraction cannot change it (torch's gradient contracts 0.5 * (1 + erf)
+// into the add, which the __fmaf_rn reproduces); erff and expf are the accurate library functions, as in torch
+__device__ __forceinline__ float gelu_f32(float x) {
+  constexpr float kAlpha = (float)M_SQRT1_2;
+  return __fmul_rn(__fmul_rn(x, 0.5f), __fadd_rn(1.f, erff(__fmul_rn(x, kAlpha))));
+}
+__device__ __forceinline__ float dgelu_f32(float dy, float x) {
+  constexpr float kAlpha = (float)M_SQRT1_2, kBeta = (float)(M_2_SQRTPI * M_SQRT1_2 * 0.5);
+  const float pdf = __fmul_rn(expf(__fmul_rn(__fmul_rn(x, -0.5f), x)), kBeta);
+  return __fmul_rn(dy, __fmaf_rn(__fadd_rn(1.f, erff(__fmul_rn(x, kAlpha))), 0.5f, __fmul_rn(x, pdf)));
+}
+__device__ __forceinline__ float round_as(TagBF16, float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
+__device__ __forceinline__ float round_as(TagF16, float v) { return __half2float(__float2half_rn(v)); }
 
 // |x| as bits: unsigned order is float order for non-negative values, with inf above every finite value and NaN
 // above inf, so a max over them is order-free and says whether the tensor was finite
@@ -129,10 +148,12 @@ struct CastArgs {
   uint32_t* counters;
   size_t M, rpb;   // rows; row tiles per block
   int K, R;        // columns; blocks per column tile
+  const void* aux; // z of FP8_ACT_DGELU, at the offsets of x
 };
 
-template <class U, class F, int L, bool BIAS>
+template <class U, class F, int L, bool BIAS, int ACT>
 __global__ void __launch_bounds__(kT) fp8_cast_kernel(CastArgs a) {
+  constexpr bool AUX = ACT == FP8_ACT_DGELU;
   constexpr bool ROWS = (L & FP8_ROWS) != 0, COLS = (L & FP8_COLS) != 0;
   __shared__ __align__(16) uint8_t tile[COLS ? kTile * kTile : 16];
   __shared__ float red[BIAS ? kPass * kTile : 1];
@@ -150,16 +171,23 @@ __global__ void __launch_bounds__(kT) fp8_cast_kernel(CastArgs a) {
 
   for (size_t mt = t0; mt < t1; ++mt) {
     const size_t r0 = mt * kTile;
-    Vec16 v[4][2];
+    Vec16 v[4][2], z[AUX ? 4 : 1][2];
 #pragma unroll
     for (int p = 0; p < 4; ++p) {
       const size_t r = r0 + p * kPass + rr;
       if (colok && r < M) {
-        const char* src = reinterpret_cast<const char*>(a.x) + (r * (size_t)K + col) * U::kBytes;
+        const size_t off = (r * (size_t)K + col) * U::kBytes;
+        const char* src = reinterpret_cast<const char*>(a.x) + off;
         v[p][0] = ld_stream16(src);
         v[p][1] = ld_stream16(src + 16);
-      } else {
+        if (AUX) {
+          const char* zs = reinterpret_cast<const char*>(a.aux) + off;
+          z[AUX ? p : 0][0] = ld_stream16(zs);
+          z[AUX ? p : 0][1] = ld_stream16(zs + 16);
+        }
+      } else {   // zeros: GELU and its gradient map them to +0, which changes neither the amax nor a sum
         v[p][0] = v[p][1] = Vec16{0, 0, 0, 0};
+        if (AUX) z[AUX ? p : 0][0] = z[AUX ? p : 0][1] = Vec16{0, 0, 0, 0};
       }
     }
 #pragma unroll
@@ -167,6 +195,16 @@ __global__ void __launch_bounds__(kT) fp8_cast_kernel(CastArgs a) {
       float f[16];
       U::unpack(v[p][0], f);
       U::unpack(v[p][1], f + 8);
+      if (ACT == FP8_ACT_GELU) {
+#pragma unroll
+        for (int k = 0; k < 16; ++k) f[k] = round_as(U{}, gelu_f32(f[k]));
+      } else if (AUX) {
+        float g[16];
+        U::unpack(z[AUX ? p : 0][0], g);
+        U::unpack(z[AUX ? p : 0][1], g + 8);
+#pragma unroll
+        for (int k = 0; k < 16; ++k) f[k] = round_as(U{}, dgelu_f32(f[k], g[k]));
+      }
 #pragma unroll
       for (int k = 0; k < 16; ++k) {
         amax = max(amax, abs_bits(f[k]));
@@ -263,29 +301,43 @@ __global__ void __launch_bounds__(kT) fp8_cast_kernel(CastArgs a) {
 
 using CastFn = void (*)(CastArgs);
 
-template <class U, class F>
-CastFn cast_kernel_uf(int layout, bool bias) {
-  switch (layout * 2 + (bias ? 1 : 0)) {
-    case FP8_ROWS * 2: return fp8_cast_kernel<U, F, FP8_ROWS, false>;
-    case FP8_ROWS * 2 + 1: return fp8_cast_kernel<U, F, FP8_ROWS, true>;
-    case FP8_COLS * 2: return fp8_cast_kernel<U, F, FP8_COLS, false>;
-    case FP8_COLS * 2 + 1: return fp8_cast_kernel<U, F, FP8_COLS, true>;
-    case FP8_BOTH * 2: return fp8_cast_kernel<U, F, FP8_BOTH, false>;
-    case FP8_BOTH * 2 + 1: return fp8_cast_kernel<U, F, FP8_BOTH, true>;
+template <class U, class F, int ACT, bool BIAS>
+CastFn cast_kernel_l(int layout) {
+  switch (layout) {
+    case FP8_ROWS: return fp8_cast_kernel<U, F, FP8_ROWS, BIAS, ACT>;
+    case FP8_COLS: return fp8_cast_kernel<U, F, FP8_COLS, BIAS, ACT>;
+    case FP8_BOTH: return fp8_cast_kernel<U, F, FP8_BOTH, BIAS, ACT>;
     default: return nullptr;
   }
 }
 
-template <class U>
-CastFn cast_kernel_u(int fmt, int layout, bool bias) {
-  if (fmt == FP8_E4M3) return cast_kernel_uf<U, E4M3>(layout, bias);
-  if (fmt == FP8_E5M2) return cast_kernel_uf<U, E5M2>(layout, bias);
+// the forward GELU has no bias gradient to produce, so it is not built with one
+template <class U, class F, int ACT>
+CastFn cast_kernel_ufa(int layout, bool bias) {
+  if constexpr (ACT == FP8_ACT_GELU)
+    return bias ? nullptr : cast_kernel_l<U, F, ACT, false>(layout);
+  else
+    return bias ? cast_kernel_l<U, F, ACT, true>(layout) : cast_kernel_l<U, F, ACT, false>(layout);
+}
+
+template <class U, class F>
+CastFn cast_kernel_uf(int layout, bool bias, int act) {
+  if (act == FP8_ACT_NONE) return cast_kernel_ufa<U, F, FP8_ACT_NONE>(layout, bias);
+  if (act == FP8_ACT_GELU) return cast_kernel_ufa<U, F, FP8_ACT_GELU>(layout, bias);
+  if (act == FP8_ACT_DGELU) return cast_kernel_ufa<U, F, FP8_ACT_DGELU>(layout, bias);
   return nullptr;
 }
 
-CastFn cast_kernel(int dtype, int fmt, int layout, bool bias) {
-  if (dtype == WIRE_BF16) return cast_kernel_u<TagBF16>(fmt, layout, bias);
-  if (dtype == WIRE_F16) return cast_kernel_u<TagF16>(fmt, layout, bias);
+template <class U>
+CastFn cast_kernel_u(int fmt, int layout, bool bias, int act) {
+  if (fmt == FP8_E4M3) return cast_kernel_uf<U, E4M3>(layout, bias, act);
+  if (fmt == FP8_E5M2) return cast_kernel_uf<U, E5M2>(layout, bias, act);
+  return nullptr;
+}
+
+CastFn cast_kernel(int dtype, int fmt, int layout, bool bias, int act) {
+  if (dtype == WIRE_BF16) return cast_kernel_u<TagBF16>(fmt, layout, bias, act);
+  if (dtype == WIRE_F16) return cast_kernel_u<TagF16>(fmt, layout, bias, act);
   return nullptr;
 }
 
@@ -317,10 +369,20 @@ int resident(Fn kernel, int* cache) {
   return n;
 }
 
-int cast_wave(int dtype, int fmt, int layout, bool bias) {
-  static int cache[2][2][4][2][kMaxDevices];
+// each activation is its own instantiation, with its own registers and so its own resident count
+int cast_wave(int dtype, int fmt, int layout, bool bias, int act) {
+  static int cache[3][2][2][4][2][kMaxDevices];
   const int d = dtype == WIRE_F16 ? 1 : 0;
-  return resident(cast_kernel(dtype, fmt, layout, bias), cache[d][fmt][layout][bias ? 1 : 0]) * sm_count();
+  return resident(cast_kernel(dtype, fmt, layout, bias, act), cache[act][d][fmt][layout][bias ? 1 : 0]) *
+         sm_count();
+}
+
+// the wave a cast's grid is planned for.  A bias gradient's fp32 sums follow the grid (row tiles per block, blocks
+// per column tile), so a cast with a prologue plans the plain cast's grid and its bias gradient is bit for bit that
+// of the plain cast of the activation; the gradient prologue, at half the plain cast's resident blocks, then runs it
+// in two waves.  Without a bias gradient every cast fills its own resident wave.
+int plan_wave(int dtype, int fmt, int layout, bool bias, int act) {
+  return cast_wave(dtype, fmt, layout, bias, bias ? FP8_ACT_NONE : act);
 }
 
 int amax_wave(int dtype) {
@@ -345,20 +407,21 @@ int amax_grid(size_t nvec, int wave) {
   return (int)(want < (size_t)wave ? want : (size_t)wave);
 }
 
-bool bad_cast_args(int dtype, int fmt, int layout) {
+bool bad_cast_args(int dtype, int fmt, int layout, int act, bool dbias) {
   return (dtype != WIRE_BF16 && dtype != WIRE_F16) || (fmt != FP8_E4M3 && fmt != FP8_E5M2) || layout < FP8_ROWS ||
-         layout > FP8_BOTH;
+         layout > FP8_BOTH || act < FP8_ACT_NONE || act > FP8_ACT_DGELU || (act == FP8_ACT_GELU && dbias);
 }
 
 }  // namespace
 
-void fp8_cast_workspace(size_t M, int K, int dtype, int fmt, int layout, bool dbias, size_t* floats, int* counters) {
+void fp8_cast_workspace(size_t M, int K, int dtype, int fmt, int layout, bool dbias, int act, size_t* floats,
+                        int* counters) {
   *floats = 0;
   *counters = 0;
-  if (bad_shape(M, K) || bad_cast_args(dtype, fmt, layout)) return;
+  if (bad_shape(M, K) || bad_cast_args(dtype, fmt, layout, act, dbias)) return;
   int nct, R;
   size_t rpb;
-  cast_grid(M, K, cast_wave(dtype, fmt, layout, dbias), &nct, &R, &rpb);
+  cast_grid(M, K, plan_wave(dtype, fmt, layout, dbias, act), &nct, &R, &rpb);
   const size_t G = (size_t)nct * R, ngroups = (size_t)nct * ((R + kGroup - 1) / kGroup);
   *floats = G + (dbias ? (G + ngroups) * kTile : 0);
   *counters = 1 + (dbias ? (int)(ngroups + nct) : 0);
@@ -390,18 +453,19 @@ cudaError_t launch_fp8_amax(const void* x, int dtype, size_t M, int K, int fmt, 
 
 cudaError_t launch_fp8_cast(const void* x, int dtype, size_t M, int K, int fmt, int layout, Fp8State* state,
                             void* out_rows, void* out_cols, float* inv, void* dbias, float* ws, uint32_t* counters,
-                            cudaStream_t s) {
-  if (bad_shape(M, K) || bad_cast_args(dtype, fmt, layout) || x == nullptr || !aligned16(x) || state == nullptr ||
-      inv == nullptr || ws == nullptr || counters == nullptr ||
+                            cudaStream_t s, int act, const void* aux) {
+  if (bad_shape(M, K) || bad_cast_args(dtype, fmt, layout, act, dbias != nullptr) || x == nullptr ||
+      !aligned16(x) || state == nullptr || inv == nullptr || ws == nullptr || counters == nullptr ||
+      (act == FP8_ACT_DGELU ? aux == nullptr || !aligned16(aux) : aux != nullptr) ||
       ((layout & FP8_ROWS) && (out_rows == nullptr || !aligned16(out_rows))) ||
       ((layout & FP8_COLS) && (out_cols == nullptr || !aligned16(out_cols))))
     return cudaErrorInvalidValue;
   const bool bias = dbias != nullptr;
   int nct, R;
   size_t rpb;
-  cast_grid(M, K, cast_wave(dtype, fmt, layout, bias), &nct, &R, &rpb);
-  CastArgs a{x, state, (uint8_t*)out_rows, (uint8_t*)out_cols, inv, dbias, ws, counters, M, rpb, K, R};
-  cast_kernel(dtype, fmt, layout, bias)<<<nct * R, kT, 0, s>>>(a);
+  cast_grid(M, K, plan_wave(dtype, fmt, layout, bias, act), &nct, &R, &rpb);
+  CastArgs a{x, state, (uint8_t*)out_rows, (uint8_t*)out_cols, inv, dbias, ws, counters, M, rpb, K, R, aux};
+  cast_kernel(dtype, fmt, layout, bias, act)<<<nct * R, kT, 0, s>>>(a);
   return cudaGetLastError();
 }
 

@@ -15,6 +15,11 @@
 //              Its last block writes *inv = 1 / scale (the inverse scale this call applied; NaN when a is not
 //              finite) and, when a is finite, hist[count % 16] = a, ++count and the next scale from the history.
 //              A non-finite a leaves the state as it was.
+//              act applies an elementwise prologue to what is read, before everything above, its result rounded to
+//              the input dtype first: FP8_ACT_GELU x -> gelu(x) (erf form), FP8_ACT_DGELU x -> the GELU gradient
+//              dx * gelu'(z), z read from aux at the same offsets (aux: [M, K] in the input dtype, 16-byte aligned;
+//              null for the other two).  FP8_ACT_GELU takes no dbias.  Both compute exactly what torch's gelu / gelu_backward kernels write, so a
+//              fused cast equals the cast of the torch op's output bit for bit.
 //   Both need fp8_workspace(...) floats of workspace and zeroed uint32 counters, not shared by two launches that can
 //   be in flight at the same time.
 #pragma once
@@ -34,15 +39,17 @@ struct Fp8State {
 
 enum Fp8Format : int { FP8_E4M3 = 0, FP8_E5M2 = 1 };
 enum Fp8Layout : int { FP8_ROWS = 1, FP8_COLS = 2, FP8_BOTH = 3 };
+enum Fp8Act : int { FP8_ACT_NONE = 0, FP8_ACT_GELU = 1, FP8_ACT_DGELU = 2 };
 
-// (fp32 workspace floats, zeroed uint32 counters) of one fp8_cast (dbias or not) / fp8_amax launch
-void fp8_cast_workspace(size_t M, int K, int dtype, int fmt, int layout, bool dbias, size_t* floats, int* counters);
+// (fp32 workspace floats, zeroed uint32 counters) of one fp8_cast (dbias or not, act) / fp8_amax launch
+void fp8_cast_workspace(size_t M, int K, int dtype, int fmt, int layout, bool dbias, int act, size_t* floats,
+                        int* counters);
 void fp8_amax_workspace(size_t M, int K, int dtype, size_t* floats, int* counters);
 
 cudaError_t launch_fp8_amax(const void* x, int dtype, size_t M, int K, int fmt, Fp8State* state, float* ws,
                             uint32_t* counters, cudaStream_t s);
 cudaError_t launch_fp8_cast(const void* x, int dtype, size_t M, int K, int fmt, int layout, Fp8State* state,
                             void* out_rows, void* out_cols, float* inv, void* dbias, float* ws, uint32_t* counters,
-                            cudaStream_t s);
+                            cudaStream_t s, int act = FP8_ACT_NONE, const void* aux = nullptr);
 
 }  // namespace bps

@@ -8,7 +8,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from ..ops.fp8 import Fp8Linear
+from ..ops.fp8 import Fp8Linear, fp8_gelu_mlp
 from ..ops.ln import DropoutAddLayerNorm
 from ..ops.xent import softmax_cross_entropy
 
@@ -31,7 +31,8 @@ class BertConfig:
     # low-precision logits in place of the fp32 cast and log-softmax of F.cross_entropy (same value)
     fused_loss: bool = False
     # qkv, proj, fc1 and fc2 of every encoder layer as ops.fp8.Fp8Linear: FP8 GEMMs with delayed scaling on sm_90
-    # (same parameters and state_dict as nn.Linear); the heads stay in the model's dtype
+    # (same parameters and state_dict as nn.Linear); the heads stay in the model's dtype.  The GELU between fc1 and
+    # fc2 then runs inside the FP8 casts (ops.fp8.fp8_gelu_mlp), with the same results
     fp8_linear: bool = False
 
 
@@ -79,10 +80,14 @@ class BertLayer(nn.Module):
         a = a.transpose(1, 2).reshape(b, s, e)
         if self.fused_norm:
             x = self.norm1(self.proj(a), x)
-            return self.norm2(self.fc2(F.gelu(self.fc1(x))), x)
+            return self.norm2(self.mlp(x), x)
         x = self.norm1(x + F.dropout(self.proj(a), self.p, self.training))
-        y = self.fc2(F.gelu(self.fc1(x)))
-        return self.norm2(x + F.dropout(y, self.p, self.training))
+        return self.norm2(x + F.dropout(self.mlp(x), self.p, self.training))
+
+    def mlp(self, x):
+        if isinstance(self.fc1, Fp8Linear):
+            return fp8_gelu_mlp(x, self.fc1, self.fc2)
+        return self.fc2(F.gelu(self.fc1(x)))
 
 
 class BertForPreTraining(nn.Module):
