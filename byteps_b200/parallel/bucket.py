@@ -110,6 +110,8 @@ class Bucket:
     priority: int = 0                                  # max priority of the parameters inside (scheduling)
     ring_cls: Optional[tuple] = None                   # (wire code, ring kind) of the ring table it belongs to
     ring_pos: int = -1                                 # position inside that table
+    lamb_win_off: int = -1                             # byte offset of the LAMB norm window (fused LAMB)
+    lamb_params: Optional[torch.Tensor] = None         # LAMB: (start, numel) per parameter, int64 on the device
 
     @property
     def nbytes(self) -> int:
@@ -142,7 +144,7 @@ class BucketedGradSync:
         init_scale, growth_factor, backoff_factor and growth_interval (see `_issue_scaled_step`)."""
         self.engine = engine
         self.world, self.rank = engine.size, engine.rank
-        self.fused = fused                     # None | "sgd" | "adam" | "adamw"
+        self.fused = fused                     # None | "sgd" | "adam" | "adamw" | "lamb"
         if loss_scaler is not None and not fused:
             raise ValueError("dynamic loss scaling needs the fused optimizer")
         self.loss_scaler = dict(loss_scaler) if loss_scaler is not None else None
@@ -187,6 +189,13 @@ class BucketedGradSync:
             for b in self.buckets:
                 b.param_off = off
                 off = (off + b.nbytes + 255) // 256 * 256
+        if fused == "lamb":
+            # every rank stores its partial norms of each parameter into its slot of every peer's window
+            from .. import _native
+
+            for b in self.buckets:
+                b.lamb_win_off = off
+                off += (_native.cuda().lamb_window_bytes(len(b.params), self.world) + 255) // 256 * 256
         self.stage_off = off
         self.stage_bytes = 0
         if self._needs_stage():
@@ -300,6 +309,31 @@ class BucketedGradSync:
         self._hp_dev = torch.zeros((ng, 64), dtype=torch.uint8, device=self.device)
         self._group_step = [0] * ng      # steps run (with dynamic loss scaling: attempted, skipped ones included)
         self.loss_scale = 1.0
+        if kind == "lamb":
+            self._init_lamb()
+
+    def _init_lamb(self):
+        """LAMB's device memory besides the Adam state: a (start, numel) table per bucket, the float64 scratch of the
+        partial norms and one float trust ratio per parameter.  The buckets of a step run in order on the comm stream,
+        so the scratch and the ratios of the largest bucket serve them all."""
+        cu = self.ctx.cu
+        cu.lamb_load_kernels()           # loaded before any launch that spins on a peer (DESIGN 1.6)
+        for b in self.buckets:
+            b.lamb_params = torch.tensor([[st, p.numel()] for p, st in zip(b.params, b.starts)], dtype=torch.int64,
+                                         device=self.device)
+        nmax = max(len(b.params) for b in self.buckets)
+        shard_max = max(s1 - s0 for s0, s1 in map(self.shard_range, self.buckets))
+        self._lamb_scratch = torch.zeros(cu.lamb_scratch_bytes(shard_max, nmax) // 8, dtype=torch.float64,
+                                         device=self.device)
+        self._lamb_phi = torch.ones(nmax, dtype=torch.float32, device=self.device)
+
+    def lamb_device_bytes(self) -> int:
+        """Device bytes fused LAMB adds to fused Adam on this rank: tables, scratch, trust ratios, norm windows."""
+        if self.fused != "lamb":
+            return 0
+        windows = sum(self.ctx.cu.lamb_window_bytes(len(b.params), self.world) for b in self.buckets)
+        return (sum(b.lamb_params.nbytes for b in self.buckets) + self._lamb_scratch.nbytes + self._lamb_phi.nbytes
+                + windows)
 
     # ------------------------------------------------------------------ dynamic loss scaling (fused mode)
     def _init_loss_scaler(self):
@@ -397,9 +431,10 @@ class BucketedGradSync:
                         int(bool(g.get("nesterov", False))), 0, int(t == 1), 1.0 / self.loss_scale, 0, 0, 0)
             else:
                 b1, b2 = g.get("betas", (0.9, 0.999))
+                adapt = int(bool(g.get("adapt", True))) if self.fused == "lamb" else 0
                 vals = (float(g.get("lr", 0.0)), float(g.get("weight_decay", 0.0)), 0.0, 0.0, float(b1), float(b2),
                         float(g.get("eps", 1e-8)), 1.0 - b1 ** t, 1.0 - b2 ** t, 0,
-                        int(self.fused == "adamw"), int(t == 1), 1.0 / self.loss_scale, 0, 0, 0)
+                        int(self.fused == "adamw"), int(t == 1), 1.0 / self.loss_scale, 0, adapt, 0)
             blob += struct.pack(_HP_FMT, *vals)
         self.ctx.cu.write_blob(self._hp_dev.data_ptr(), blob, cur.cuda_stream)
         self.engine.launches += 1
@@ -502,6 +537,10 @@ class BucketedGradSync:
         shard = (wbytes + world - 1) // world
         blocks = self.engine.cfg.comm_blocks or pick_blocks(shard, self.threads, 32, cap=64)
         nvls = self._nvls_for(wire)
+        if self.fused == "lamb":
+            self._launch_lamb(b, wire, scale, blocks, nvls, cs)
+            self._after_launch(b, cur, cs, ev_t)
+            return
         if self.fused:
             kind = cu.OPT_SGD if self.fused == "sgd" else cu.OPT_ADAM
             hp_ptr = self._hp_dev.data_ptr() + 64 * b.group_index
@@ -551,6 +590,28 @@ class BucketedGradSync:
                                cs.cuda_stream)
         self._after_launch(b, cur, cs, ev_t)
 
+    def _launch_lamb(self, b: Bucket, wire, scale, blocks, nvls, cs):
+        """LAMB: three kernels per bucket (pushpull_lamb.cuh).  lamb_moments reduces this rank's shard, updates the
+        moments and sums w^2 and u^2 per parameter; lamb_norms trades those sums with the peers and forms the trust
+        ratios; lamb_apply updates the masters and all-gathers the parameters.  The grids depend on the bucket only."""
+        cu = self.ctx.cu
+        if wire == b.dtype:
+            segs, nsegs, stage = 0, 0, b.grad_off
+        else:
+            segs, nsegs, stage = self._seg_table(b).data_ptr(), 1, self.stage_off
+        hp = self._hp_dev.data_ptr() + 64 * b.group_index
+        n, table = len(b.params), b.lamb_params.data_ptr()
+        scratch, phi = self._lamb_scratch.data_ptr(), self._lamb_phi.data_ptr()
+        g, w = wire_code(b.dtype), wire_code(wire)
+        cu.lamb_moments(self.ctx.view, g, w, segs, nsegs, stage, b.numel, scale, b.master.data_ptr(),
+                        b.state0.data_ptr(), b.state1.data_ptr(), table, n, scratch, hp, blocks, self.threads, 0, nvls,
+                        cs.cuda_stream)
+        cu.lamb_norms(self.ctx.view, w, b.numel, table, n, scratch, b.lamb_win_off, phi, hp, min(n, 32), 0,
+                      cs.cuda_stream)
+        cu.lamb_apply(self.ctx.view, g, w, b.param_off, b.numel, b.master.data_ptr(), b.state0.data_ptr(),
+                      b.state1.data_ptr(), table, n, phi, hp, blocks, self.threads, 0, nvls, cs.cuda_stream)
+        self._count_launch(2)            # _after_launch counts the third
+
     # ------------------------------------------------------------------ descriptor ring
     def _setup_ring(self):
         """BYTEPS_RING: how bucket exchanges reach the GPU.
@@ -586,7 +647,9 @@ class BucketedGradSync:
         self._ring_credit = credit * self.engine.cfg.partition_bound() if credit > 0 else 0
         self._stamps = os.environ.get("BYTEPS_COMM_STAMPS", "1") not in ("0", "")
         self._stamp_base = None
+        # LAMB needs every rank's partial norms between the reduction and the update: per-bucket launches only
         eligible = (self._reduce_engine in ("auto", "nvls", "lsu") and len(self.buckets) <= cu.RING_SLOTS
+                    and self.fused != "lamb"
                     and not (self.fused and self._fused_engine == "tma" and self.world == 1 and mode == "auto"))
         if mode == "auto":
             # one rank: nothing to wait for, the TMA-streamed optimizer kernel per bucket is the fastest;

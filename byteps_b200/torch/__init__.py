@@ -11,7 +11,7 @@ What is different underneath: on CUDA the optimizer does not issue one
 push_pull per parameter.  Gradients live in a symmetric NVLink-mapped arena and
 are exchanged bucket by bucket by one fused sm_90a kernel each
 (:mod:`byteps_b200.parallel.bucket`); with ``fused_update=True`` the kernel also
-applies the SGD/Adam step on fp32 master weights and all-gathers the new
+applies the SGD/Adam/LAMB step on fp32 master weights and all-gathers the new
 parameters instead of the gradients.
 """
 from __future__ import annotations
@@ -27,6 +27,7 @@ import torch
 from ..common import config as _config
 from ..common import engine as _engine
 from .compression import Compression
+from .lamb import Lamb
 from .ops import (byteps_torch_set_num_grads, declare, get_pushpull_speed, init, local_rank, local_size, poll,
                   push_pull, push_pull_async, push_pull_async_inplace, push_pull_group_sync_inplace,
                   push_pull_inplace, rank, resume, set_learning_rate, shutdown, size, suspend, synchronize)
@@ -37,6 +38,7 @@ __all__ = [
     "push_pull", "push_pull_async", "push_pull_inplace", "push_pull_async_inplace", "push_pull_group_sync_inplace",
     "poll", "synchronize", "declare", "byteps_torch_set_num_grads", "DistributedOptimizer", "broadcast_parameters",
     "broadcast_optimizer_state", "broadcast_object", "Compression", "set_learning_rate", "convert_sync_batchnorm",
+    "Lamb",
 ]
 
 
@@ -50,6 +52,8 @@ def _wire_of(compression):
 
 def _fused_kind(optimizer_cls, param_groups):
     name = optimizer_cls.__name__
+    if issubclass(optimizer_cls, Lamb):
+        return "lamb"
     if issubclass(optimizer_cls, torch.optim.SGD):
         return "sgd"
     if issubclass(optimizer_cls, torch.optim.AdamW):
@@ -181,7 +185,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
 
             kind = _fused_kind(self.__class__.__mro__[1], self.param_groups) if fused_update else None
             if fused_update and kind is None:
-                raise ValueError("fused_update supports SGD, Adam and AdamW (no amsgrad)")
+                raise ValueError("fused_update supports SGD, Adam, AdamW (no amsgrad) and byteps_b200.torch.Lamb")
             self._fused = kind
             self._sync = BucketedGradSync(eng, self.param_groups, fused=kind, wire_dtype=_wire_of(compression),
                                           bucket_bytes=bucket_bytes,
@@ -367,9 +371,10 @@ class _DistributedOptimizer(torch.optim.Optimizer):
 
     # ---- checkpoints of the fused optimizer ----------------------------------------
     # With fused_update the state lives in the exchange's fp32 shards, not in self.state.  state_dict() gathers it
-    # into the layout torch.optim uses (SGD: momentum_buffer; Adam/AdamW: step, exp_avg, exp_avg_sq), plus
+    # into the layout torch.optim uses (SGD: momentum_buffer; Adam/AdamW/Lamb: step, exp_avg, exp_avg_sq), plus
     # master_param for 16-bit parameters; load_state_dict() takes that layout, from this class or from torch.optim.
-    _FUSED_KEYS = {"sgd": ("momentum_buffer",), "adam": ("exp_avg", "exp_avg_sq"), "adamw": ("exp_avg", "exp_avg_sq")}
+    _FUSED_KEYS = {"sgd": ("momentum_buffer",), "adam": ("exp_avg", "exp_avg_sq"), "adamw": ("exp_avg", "exp_avg_sq"),
+                   "lamb": ("exp_avg", "exp_avg_sq")}
 
     def state_dict(self):
         """The optimizer state in ``torch.optim``'s format.
@@ -480,7 +485,8 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
 
     Arguments match the reference (optimizer, named_parameters, compression,
     backward_passes_per_step).  Extras: ``fused_update=True`` applies the
-    SGD/Adam(W) step on fp32 master weights inside the exchange kernel;
+    SGD, Adam(W) or :class:`Lamb` step on fp32 master weights inside the
+    exchange kernels;
     ``bucket_bytes`` sets the fusion granularity; ``compression_params`` (e.g.
     ``{"compressor": "topk", "k": 0.01, "ef": "vanilla"}``, docs/gradient-compression.md)
     turns on lossy gradient compression per tensor - GPU kernels over NVLink, or the

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """BERT-large pre-training step loop (the reference's bandwidth-bound headline
-workload) with the fused Adam exchange: bf16 parameters/gradients, fp32 master
-weights and moments sharded over the GPUs, one kernel per bucket."""
+workload) with the fused AdamW or LAMB exchange: bf16 parameters/gradients, fp32
+master weights and moments sharded over the GPUs, updated inside the exchange."""
 import argparse
 import os
 import sys
@@ -26,6 +26,8 @@ p.add_argument("--fused-loss", action="store_true",
                help="fused softmax cross-entropy kernels for the masked-LM loss")
 p.add_argument("--fp8-linear", action="store_true",
                help="FP8 GEMMs with delayed scaling for the encoder layers' linear layers (sm_90)")
+p.add_argument("--optimizer", choices=("adamw", "lamb"), default="adamw",
+               help="lamb: weights with decay and the trust ratio; biases and LayerNorm weights without either")
 args = p.parse_args()
 bps.init()
 cuda = torch.cuda.is_available() and not args.no_cuda
@@ -36,8 +38,15 @@ model = get_model(args.model, fused_norm=args.fused_norm, fused_loss=args.fused_
                   fp8_linear=args.fp8_linear).to(dev)
 if cuda:
     model = model.to(torch.bfloat16)
-opt = bps.DistributedOptimizer(torch.optim.AdamW(model.parameters(), lr=1e-4, weight_decay=0.01),
-                               named_parameters=model.named_parameters(), fused_update=cuda)
+if args.optimizer == "lamb":
+    # the usual BERT split: 1-D parameters (biases, LayerNorm weights) take neither decay nor adaptation
+    decay = [p for p in model.parameters() if p.dim() > 1]
+    plain = [p for p in model.parameters() if p.dim() <= 1]
+    inner = bps.Lamb([dict(params=decay, weight_decay=0.01),
+                      dict(params=plain, weight_decay=0.0, adapt=False)], lr=1e-3)
+else:
+    inner = torch.optim.AdamW(model.parameters(), lr=1e-4, weight_decay=0.01)
+opt = bps.DistributedOptimizer(inner, named_parameters=model.named_parameters(), fused_update=cuda)
 bps.broadcast_parameters(model.state_dict(), root_rank=0)
 ids = torch.randint(0, 30522, (args.batch_size, args.seq_len), device=dev)
 labels = torch.randint(0, 30522, (args.batch_size, args.seq_len), device=dev)
