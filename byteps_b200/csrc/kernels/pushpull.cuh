@@ -47,8 +47,8 @@ struct OptHParams {
   int first_step;    // momentum buffer initialisation (buf = g)
   float grad_scale;  // extra multiplier on the reduced gradient (loss-scale^-1)
   int skip;          // dynamic loss scaling found an overflow: leave the optimizer state as it is
-  int adapt;         // LAMB: scale the update by the trust ratio ||w|| / ||u|| (0: ratio 1)
-  int pad;
+  int adapt;         // LAMB / LARS: scale the update by the trust ratio (0: ratio 1)
+  float trust_coefficient;  // LARS: eta of phi = eta * ||w|| / (||g|| + wd * ||w|| + eps)
 };
 
 struct LaunchCfg {

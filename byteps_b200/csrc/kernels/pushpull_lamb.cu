@@ -1,42 +1,19 @@
 // LAMB in the fused exchange: the three kernels of a bucket (see pushpull_lamb.cuh for the sequence).
 //
 // The shard geometry, the pack phase, the peer reduction and the all-gather sink are those of the fused Adam kernel
-// (pushpull_dev.cuh).  Grids depend on the bucket only: lamb_moments and lamb_apply take the bucket's CTA count,
+// (pushpull_dev.cuh); the parameter cursor, the segmented warp sums and the norm exchange are shared with LARS
+// (pushpull_trust.cuh).  Grids depend on the bucket only: lamb_moments and lamb_apply take the bucket's CTA count,
 // lamb_norms one CTA per parameter up to its cap, so barrier_peers pairs the same CTA index on every rank, a rank
 // with an empty shard included.
 #include "kernels/pushpull_lamb.cuh"
 
 #include "kernels/common.cuh"
 #include "kernels/pushpull_dev.cuh"
+#include "kernels/pushpull_trust.cuh"
 
 namespace bps {
 
 namespace {
-
-constexpr int kNormThreads = 256;
-constexpr unsigned kFull = 0xffffffffu;
-
-// The parameter that holds flat element e: the last one whose start is <= e (its padding included).  Each thread
-// visits its units in increasing order, so after one binary search the cursor only moves forward.
-struct ParamCursor {
-  const LambParam* params;
-  int n;
-  int i;
-  __device__ __forceinline__ void init(const LambParam* p, int np, int64_t e) {
-    params = p;
-    n = np;
-    int lo = 0, hi = np - 1;
-    while (lo < hi) {
-      const int mid = (lo + hi + 1) >> 1;
-      if (__ldg(&params[mid].start) <= e) lo = mid;
-      else hi = mid - 1;
-    }
-    i = lo;
-  }
-  __device__ __forceinline__ void seek(int64_t e) {
-    while (i + 1 < n && __ldg(&params[i + 1].start) <= e) ++i;
-  }
-};
 
 // u of one element from the updated moments and the master before the update.  lamb_moments (for the norm) and
 // lamb_apply (for the step) both call this with the same inputs; the rounding steps are spelled out so the two
@@ -81,24 +58,13 @@ __global__ void __launch_bounds__(512) lamb_moments_kernel(PeerView pv, const Se
     if (nvls) {
       if (valid) W::unpack(W::mm_reduce(pv.mc_data + stage_off + unit * 16), g);
     } else {
-      const size_t idx[1] = {unit};
-      const bool vld[1] = {valid};
-      float acc[1][E];
-      reduce_units_p2p<W, 1>(pv, stage_off, idx, vld, rot, acc);
-#pragma unroll
-      for (int k = 0; k < E; ++k) g[k] = acc[0][k];
+      reduce_unit_p2p<W>(pv, stage_off, unit, valid, rot, g);
     }
     double w2 = 0.0, u2 = 0.0;
     int pid = -1;
     if (valid) {
       const int64_t e = (int64_t)(unit * E);
-      if (!inited) {
-        cur.init(params, nparams, e);
-        inited = true;
-      } else {
-        cur.seek(e);
-      }
-      pid = cur.i;
+      pid = cur.at(params, nparams, e, inited);
       const int64_t end = __ldg(&params[pid].start) + __ldg(&params[pid].n);
 #pragma unroll
       for (int k = 0; k < E; ++k) {
@@ -114,21 +80,7 @@ __global__ void __launch_bounds__(512) lamb_moments_kernel(PeerView pv, const Se
       stf<E>(m1 + li, m);
       stf<E>(m2 + li, v);
     }
-    // Segmented suffix sums over the warp's 32 units: a parameter's units are contiguous, so after the five steps
-    // the first lane of each segment holds the segment's sum, added in a fixed order.
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const double ow = __shfl_down_sync(kFull, w2, off);
-      const double ou = __shfl_down_sync(kFull, u2, off);
-      const int op = __shfl_down_sync(kFull, pid, off);
-      if (lane + off < 32 && op == pid) {
-        w2 += ow;
-        u2 += ou;
-      }
-    }
-    const int prev = __shfl_up_sync(kFull, pid, 1);
-    if (valid && (lane == 0 || prev != pid))
-      (lane == 0 ? groups[(unit - s0) / 32] : heads[pid]) = make_double2(w2, u2);
+    BPS_STORE_SEGMENT_SUMS(w2, u2, pid, valid, lane, unit, s0, groups, heads);
   });
 }
 
@@ -137,54 +89,10 @@ __global__ void __launch_bounds__(kNormThreads) lamb_norms_kernel(PeerView pv, s
                                                                   const LambParam* params, int nparams,
                                                                   const double* scratch, size_t win_off, float* phi,
                                                                   const OptHParams* hpp, int channel) {
-  __shared__ double2 red[kNormThreads];
-  const bool skip = hpp->skip != 0;
-  size_t s0, s1;
-  shard_units_of<E>(total_groups, pv.world, pv.rank, &s0, &s1);
-  const double2* heads = reinterpret_cast<const double2*>(scratch);
-  const double2* groups = heads + nparams;
-  for (int p = blockIdx.x; p < nparams; p += gridDim.x) {
-    const int64_t st = params[p].start;
-    const size_t ua = (size_t)st / E, ub = (size_t)(st + (params[p].n + 7) / 8 * 8) / E;
-    const size_t a = ua > s0 ? ua : s0, b = ub < s1 ? ub : s1;
-    double2 acc = make_double2(0.0, 0.0);
-    if (!skip && a < b) {
-      // the warp segments of the parameter in this shard: those that begin a 32-unit group, in unit order per
-      // thread, and the one that begins at the parameter's first unit inside a group
-      const size_t g0 = (a - s0 + 31) / 32, g1 = (b - s0 + 31) / 32;
-      for (size_t gi = g0 + threadIdx.x; gi < g1; gi += blockDim.x) {
-        acc.x += groups[gi].x;
-        acc.y += groups[gi].y;
-      }
-      if (threadIdx.x == 0 && a == ua && ((a - s0) & 31)) {
-        acc.x += heads[p].x;
-        acc.y += heads[p].y;
-      }
-    }
-    red[threadIdx.x] = acc;
-    __syncthreads();
-    for (int s = kNormThreads / 2; s > 0; s >>= 1) {
-      if (threadIdx.x < s) {
-        red[threadIdx.x].x += red[threadIdx.x + s].x;
-        red[threadIdx.x].y += red[threadIdx.x + s].y;
-      }
-      __syncthreads();
-    }
-    if (!skip && threadIdx.x < pv.world)
-      reinterpret_cast<double2*>(pv.data[threadIdx.x] + win_off)[(size_t)p * pv.world + pv.rank] = red[0];
-    __syncthreads();
-  }
-  barrier_peers(pv, channel);   // the peers' CTA of this index has stored the same parameters' slots
-  if (skip) return;
-  const volatile double* win = reinterpret_cast<const volatile double*>(pv.data[pv.rank] + win_off);
-  for (int p = blockIdx.x + threadIdx.x * gridDim.x; p < nparams; p += gridDim.x * blockDim.x) {
-    double ws = 0.0, us = 0.0;
-    for (int r = 0; r < pv.world; ++r) {
-      ws += win[((size_t)p * pv.world + r) * 2];
-      us += win[((size_t)p * pv.world + r) * 2 + 1];
-    }
-    phi[p] = (hpp->adapt && ws > 0.0 && us > 0.0) ? (float)(sqrt(ws) / sqrt(us)) : 1.f;
-  }
+  exchange_norms<E>(pv, total_groups, params, nparams, scratch, win_off, phi, hpp->skip != 0, channel,
+                    [&](double ws, double us) {
+                      return (hpp->adapt && ws > 0.0 && us > 0.0) ? (float)(sqrt(ws) / sqrt(us)) : 1.f;
+                    });
 }
 
 template <class W, class P>
@@ -210,34 +118,13 @@ __global__ void __launch_bounds__(512) lamb_apply_kernel(PeerView pv, size_t par
     ldf<E>(m1 + li, m);
     ldf<E>(m2 + li, v);
     const int64_t e = (int64_t)(unit * E);
-    if (!inited) {
-      cur.init(params, nparams, e);
-      inited = true;
-    } else {
-      cur.seek(e);
-    }
-    const float lr_phi = hp.lr * __ldg(&phi[cur.i]);
+    const float lr_phi = hp.lr * __ldg(&phi[cur.at(params, nparams, e, inited)]);
 #pragma unroll
     for (int k = 0; k < E; ++k) w[k] = __fmaf_rn(-lr_phi, lamb_u(w[k], m[k], v[k], inv_c1, inv_c2, hp), w[k]);
     stf<E>(master + li, w);
     sink_peers<P, E>(pv, param_off, unit, w, nvls != 0);
   });
   barrier_peers(pv, channel);
-}
-
-inline bool bad_geometry(int blocks, int threads) {
-  return blocks < 1 || blocks > kMaxBlocks || threads < 32 || threads > 512 || (threads & 31);
-}
-
-// exactly the (gradient, wire) pairs of launch_pushpull_fused_opt; the parameters have the gradient dtype
-template <class F>
-cudaError_t dispatch_pair(int grad_dtype, int wire, F&& f) {
-  if (grad_dtype == WIRE_F32 && wire == WIRE_F32) return f(TagF32{}, TagF32{});
-  if (grad_dtype == WIRE_F32 && wire == WIRE_BF16) return f(TagF32{}, TagBF16{});
-  if (grad_dtype == WIRE_F32 && wire == WIRE_F16) return f(TagF32{}, TagF16{});
-  if (grad_dtype == WIRE_BF16 && wire == WIRE_BF16) return f(TagBF16{}, TagBF16{});
-  if (grad_dtype == WIRE_F16 && wire == WIRE_F16) return f(TagF16{}, TagF16{});
-  return cudaErrorInvalidValue;
 }
 
 }  // namespace

@@ -110,8 +110,8 @@ class Bucket:
     priority: int = 0                                  # max priority of the parameters inside (scheduling)
     ring_cls: Optional[tuple] = None                   # (wire code, ring kind) of the ring table it belongs to
     ring_pos: int = -1                                 # position inside that table
-    lamb_win_off: int = -1                             # byte offset of the LAMB norm window (fused LAMB)
-    lamb_params: Optional[torch.Tensor] = None         # LAMB: (start, numel) per parameter, int64 on the device
+    lamb_win_off: int = -1                             # byte offset of the norm window (fused LAMB and LARS)
+    lamb_params: Optional[torch.Tensor] = None         # LAMB, LARS: (start, numel) per parameter, int64 on the device
 
     @property
     def nbytes(self) -> int:
@@ -129,7 +129,8 @@ def resync_fused_masters():
             s.sync_master_from_params()
 
 
-_HP_FMT = "<9f3if3i"   # matches csrc/kernels/pushpull.cuh::OptHParams (64 bytes)
+_HP_FMT = "<9f3if2if"   # matches csrc/kernels/pushpull.cuh::OptHParams (64 bytes)
+_TRUST_KINDS = ("lamb", "lars")   # fused optimizers with per-parameter trust ratios: three launches per bucket
 _LS_STATE_FMT = "<2df5i"   # csrc/kernels/loss_scale.cuh::LossScaleState (40 bytes)
 _LS_ENTRY_FMT = "<2Q4i"    # csrc/kernels/loss_scale.cuh::LossScaleCheckEntry (32 bytes)
 
@@ -144,7 +145,7 @@ class BucketedGradSync:
         init_scale, growth_factor, backoff_factor and growth_interval (see `_issue_scaled_step`)."""
         self.engine = engine
         self.world, self.rank = engine.size, engine.rank
-        self.fused = fused                     # None | "sgd" | "adam" | "adamw" | "lamb"
+        self.fused = fused                     # None | "sgd" | "adam" | "adamw" | "lamb" | "lars"
         if loss_scaler is not None and not fused:
             raise ValueError("dynamic loss scaling needs the fused optimizer")
         self.loss_scaler = dict(loss_scaler) if loss_scaler is not None else None
@@ -189,7 +190,7 @@ class BucketedGradSync:
             for b in self.buckets:
                 b.param_off = off
                 off = (off + b.nbytes + 255) // 256 * 256
-        if fused == "lamb":
+        if fused in _TRUST_KINDS:
             # every rank stores its partial norms of each parameter into its slot of every peer's window
             from .. import _native
 
@@ -304,20 +305,25 @@ class BucketedGradSync:
             b.master = torch.zeros(n, dtype=torch.float32, device=self.device)
             b.master[: s1 - s0].copy_(b.flat_param[s0:s1].float())
             b.state0 = torch.zeros(n, dtype=torch.float32, device=self.device)
-            b.state1 = torch.zeros(n, dtype=torch.float32, device=self.device) if kind != "sgd" else None
+            b.state1 = torch.zeros(n, dtype=torch.float32, device=self.device) if kind not in ("sgd", "lars") else None
         ng = len(self.param_groups)
         self._hp_dev = torch.zeros((ng, 64), dtype=torch.uint8, device=self.device)
         self._group_step = [0] * ng      # steps run (with dynamic loss scaling: attempted, skipped ones included)
         self.loss_scale = 1.0
-        if kind == "lamb":
+        if kind in _TRUST_KINDS:
             self._init_lamb()
 
     def _init_lamb(self):
-        """LAMB's device memory besides the Adam state: a (start, numel) table per bucket, the float64 scratch of the
-        partial norms and one float trust ratio per parameter.  The buckets of a step run in order on the comm stream,
-        so the scratch and the ratios of the largest bucket serve them all."""
+        """The device memory of a trust-ratio optimizer (LAMB, LARS) besides its SGD or Adam state: a (start, numel)
+        table per bucket, the float64 scratch of the partial norms and one float trust ratio per parameter.  The
+        buckets of a step run in order on the comm stream, so the scratch and the ratios of the largest bucket serve
+        them all."""
         cu = self.ctx.cu
-        cu.lamb_load_kernels()           # loaded before any launch that spins on a peer (DESIGN 1.6)
+        # loaded before any launch that spins on a peer (DESIGN 1.6)
+        if self.fused == "lamb":
+            cu.lamb_load_kernels()
+        else:
+            cu.lars_load_kernels()
         for b in self.buckets:
             b.lamb_params = torch.tensor([[st, p.numel()] for p, st in zip(b.params, b.starts)], dtype=torch.int64,
                                          device=self.device)
@@ -328,8 +334,9 @@ class BucketedGradSync:
         self._lamb_phi = torch.ones(nmax, dtype=torch.float32, device=self.device)
 
     def lamb_device_bytes(self) -> int:
-        """Device bytes fused LAMB adds to fused Adam on this rank: tables, scratch, trust ratios, norm windows."""
-        if self.fused != "lamb":
+        """Device bytes fused LAMB adds to fused Adam, or fused LARS to fused SGD, on this rank: tables, scratch,
+        trust ratios, norm windows."""
+        if self.fused not in _TRUST_KINDS:
             return 0
         windows = sum(self.ctx.cu.lamb_window_bytes(len(b.params), self.world) for b in self.buckets)
         return (sum(b.lamb_params.nbytes for b in self.buckets) + self._lamb_scratch.nbytes + self._lamb_phi.nbytes
@@ -428,17 +435,21 @@ class BucketedGradSync:
             if self.fused == "sgd":
                 vals = (float(g.get("lr", 0.0)), float(g.get("weight_decay", 0.0)), float(g.get("momentum", 0.0)),
                         float(g.get("dampening", 0.0)), 0.0, 0.0, 0.0, 1.0, 1.0,
-                        int(bool(g.get("nesterov", False))), 0, int(t == 1), 1.0 / self.loss_scale, 0, 0, 0)
+                        int(bool(g.get("nesterov", False))), 0, int(t == 1), 1.0 / self.loss_scale, 0, 0, 0.0)
+            elif self.fused == "lars":
+                vals = (float(g.get("lr", 0.0)), float(g.get("weight_decay", 0.0)), float(g.get("momentum", 0.0)),
+                        0.0, 0.0, 0.0, float(g.get("eps", 0.0)), 1.0, 1.0, 0, 0, int(t == 1), 1.0 / self.loss_scale,
+                        0, int(bool(g.get("adapt", True))), float(g.get("trust_coefficient", 0.001)))
             else:
                 b1, b2 = g.get("betas", (0.9, 0.999))
                 adapt = int(bool(g.get("adapt", True))) if self.fused == "lamb" else 0
                 vals = (float(g.get("lr", 0.0)), float(g.get("weight_decay", 0.0)), 0.0, 0.0, float(b1), float(b2),
                         float(g.get("eps", 1e-8)), 1.0 - b1 ** t, 1.0 - b2 ** t, 0,
-                        int(self.fused == "adamw"), int(t == 1), 1.0 / self.loss_scale, 0, adapt, 0)
+                        int(self.fused == "adamw"), int(t == 1), 1.0 / self.loss_scale, 0, adapt, 0.0)
             blob += struct.pack(_HP_FMT, *vals)
         self.ctx.cu.write_blob(self._hp_dev.data_ptr(), blob, cur.cuda_stream)
         self.engine.launches += 1
-        if self.loss_scaler is not None and self.fused != "sgd":
+        if self.loss_scaler is not None and self.fused not in ("sgd", "lars"):
             # loss_scale_update forms Adam's bias corrections on the device, from the betas as the host holds them
             betas = b"".join(struct.pack("<2d", *map(float, g.get("betas", (0.9, 0.999)))) for g in self.param_groups)
             self.ctx.cu.write_blob(self._ls_betas.data_ptr(), betas, cur.cuda_stream)
@@ -537,8 +548,8 @@ class BucketedGradSync:
         shard = (wbytes + world - 1) // world
         blocks = self.engine.cfg.comm_blocks or pick_blocks(shard, self.threads, 32, cap=64)
         nvls = self._nvls_for(wire)
-        if self.fused == "lamb":
-            self._launch_lamb(b, wire, scale, blocks, nvls, cs)
+        if self.fused in _TRUST_KINDS:
+            self._launch_trust(b, wire, scale, blocks, nvls, cs)
             self._after_launch(b, cur, cs, ev_t)
             return
         if self.fused:
@@ -590,10 +601,13 @@ class BucketedGradSync:
                                cs.cuda_stream)
         self._after_launch(b, cur, cs, ev_t)
 
-    def _launch_lamb(self, b: Bucket, wire, scale, blocks, nvls, cs):
-        """LAMB: three kernels per bucket (pushpull_lamb.cuh).  lamb_moments reduces this rank's shard, updates the
-        moments and sums w^2 and u^2 per parameter; lamb_norms trades those sums with the peers and forms the trust
-        ratios; lamb_apply updates the masters and all-gathers the parameters.  The grids depend on the bucket only."""
+    def _launch_trust(self, b: Bucket, wire, scale, blocks, nvls, cs):
+        """LAMB and LARS: three kernels per bucket.  LAMB (pushpull_lamb.cuh): lamb_moments reduces this rank's shard,
+        updates the moments and sums w^2 and u^2 per parameter; lamb_norms trades those sums with the peers and forms
+        the trust ratios; lamb_apply updates the masters and all-gathers the parameters.  LARS (pushpull_lars.cuh):
+        lars_norms_partial reduces the shard and sums w^2 and g^2; lars_norms forms the ratios as lamb_norms does;
+        lars_apply reduces the shard again, updates the momentum and the masters and all-gathers the parameters.  The
+        grids depend on the bucket only."""
         cu = self.ctx.cu
         if wire == b.dtype:
             segs, nsegs, stage = 0, 0, b.grad_off
@@ -603,6 +617,15 @@ class BucketedGradSync:
         n, table = len(b.params), b.lamb_params.data_ptr()
         scratch, phi = self._lamb_scratch.data_ptr(), self._lamb_phi.data_ptr()
         g, w = wire_code(b.dtype), wire_code(wire)
+        if self.fused == "lars":
+            cu.lars_norms_partial(self.ctx.view, g, w, segs, nsegs, stage, b.numel, scale, b.master.data_ptr(), table, n,
+                                  scratch, hp, blocks, self.threads, 0, nvls, cs.cuda_stream)
+            cu.lars_norms(self.ctx.view, w, b.numel, table, n, scratch, b.lamb_win_off, phi, hp, min(n, 32), 0,
+                          cs.cuda_stream)
+            cu.lars_apply(self.ctx.view, g, w, stage, b.param_off, b.numel, scale, b.master.data_ptr(),
+                          b.state0.data_ptr(), table, n, phi, hp, blocks, self.threads, 0, nvls, cs.cuda_stream)
+            self._count_launch(2)        # _after_launch counts the third
+            return
         cu.lamb_moments(self.ctx.view, g, w, segs, nsegs, stage, b.numel, scale, b.master.data_ptr(),
                         b.state0.data_ptr(), b.state1.data_ptr(), table, n, scratch, hp, blocks, self.threads, 0, nvls,
                         cs.cuda_stream)
@@ -647,9 +670,9 @@ class BucketedGradSync:
         self._ring_credit = credit * self.engine.cfg.partition_bound() if credit > 0 else 0
         self._stamps = os.environ.get("BYTEPS_COMM_STAMPS", "1") not in ("0", "")
         self._stamp_base = None
-        # LAMB needs every rank's partial norms between the reduction and the update: per-bucket launches only
+        # LAMB and LARS need every rank's partial norms between the reduction and the update: per-bucket launches only
         eligible = (self._reduce_engine in ("auto", "nvls", "lsu") and len(self.buckets) <= cu.RING_SLOTS
-                    and self.fused != "lamb"
+                    and self.fused not in _TRUST_KINDS
                     and not (self.fused and self._fused_engine == "tma" and self.world == 1 and mode == "auto"))
         if mode == "auto":
             # one rank: nothing to wait for, the TMA-streamed optimizer kernel per bucket is the fastest;
@@ -888,7 +911,7 @@ class BucketedGradSync:
                             cs.cuda_stream)
         cu.loss_scale_update(self.ctx.view, 0, self.ls_win_off, state, self._ls_steps.data_ptr(),
                              self._ls_betas.data_ptr(), self._hp_dev.data_ptr(), len(self.param_groups),
-                             self.fused != "sgd", cs.cuda_stream)
+                             self.fused not in ("sgd", "lars"), cs.cuda_stream)
         self._count_launch(2)
         for b in self.buckets:
             if self._ring_mode != "off" and b.ring_cls is not None:

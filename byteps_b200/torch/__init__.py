@@ -11,7 +11,7 @@ What is different underneath: on CUDA the optimizer does not issue one
 push_pull per parameter.  Gradients live in a symmetric NVLink-mapped arena and
 are exchanged bucket by bucket by one fused sm_90a kernel each
 (:mod:`byteps_b200.parallel.bucket`); with ``fused_update=True`` the kernel also
-applies the SGD/Adam/LAMB step on fp32 master weights and all-gathers the new
+applies the SGD/Adam/LAMB/LARS step on fp32 master weights and all-gathers the new
 parameters instead of the gradients.
 """
 from __future__ import annotations
@@ -28,6 +28,7 @@ from ..common import config as _config
 from ..common import engine as _engine
 from .compression import Compression
 from .lamb import Lamb
+from .lars import Lars
 from .ops import (byteps_torch_set_num_grads, declare, get_pushpull_speed, init, local_rank, local_size, poll,
                   push_pull, push_pull_async, push_pull_async_inplace, push_pull_group_sync_inplace,
                   push_pull_inplace, rank, resume, set_learning_rate, shutdown, size, suspend, synchronize)
@@ -38,7 +39,7 @@ __all__ = [
     "push_pull", "push_pull_async", "push_pull_inplace", "push_pull_async_inplace", "push_pull_group_sync_inplace",
     "poll", "synchronize", "declare", "byteps_torch_set_num_grads", "DistributedOptimizer", "broadcast_parameters",
     "broadcast_optimizer_state", "broadcast_object", "Compression", "set_learning_rate", "convert_sync_batchnorm",
-    "Lamb",
+    "Lamb", "Lars",
 ]
 
 
@@ -54,6 +55,8 @@ def _fused_kind(optimizer_cls, param_groups):
     name = optimizer_cls.__name__
     if issubclass(optimizer_cls, Lamb):
         return "lamb"
+    if issubclass(optimizer_cls, Lars):
+        return "lars"
     if issubclass(optimizer_cls, torch.optim.SGD):
         return "sgd"
     if issubclass(optimizer_cls, torch.optim.AdamW):
@@ -185,7 +188,8 @@ class _DistributedOptimizer(torch.optim.Optimizer):
 
             kind = _fused_kind(self.__class__.__mro__[1], self.param_groups) if fused_update else None
             if fused_update and kind is None:
-                raise ValueError("fused_update supports SGD, Adam, AdamW (no amsgrad) and byteps_b200.torch.Lamb")
+                raise ValueError("fused_update supports SGD, Adam, AdamW (no amsgrad), byteps_b200.torch.Lamb and "
+                                 "byteps_b200.torch.Lars")
             self._fused = kind
             self._sync = BucketedGradSync(eng, self.param_groups, fused=kind, wire_dtype=_wire_of(compression),
                                           bucket_bytes=bucket_bytes,
@@ -371,10 +375,10 @@ class _DistributedOptimizer(torch.optim.Optimizer):
 
     # ---- checkpoints of the fused optimizer ----------------------------------------
     # With fused_update the state lives in the exchange's fp32 shards, not in self.state.  state_dict() gathers it
-    # into the layout torch.optim uses (SGD: momentum_buffer; Adam/AdamW/Lamb: step, exp_avg, exp_avg_sq), plus
+    # into the layout torch.optim uses (SGD and Lars: momentum_buffer; Adam/AdamW/Lamb: step, exp_avg, exp_avg_sq), plus
     # master_param for 16-bit parameters; load_state_dict() takes that layout, from this class or from torch.optim.
     _FUSED_KEYS = {"sgd": ("momentum_buffer",), "adam": ("exp_avg", "exp_avg_sq"), "adamw": ("exp_avg", "exp_avg_sq"),
-                   "lamb": ("exp_avg", "exp_avg_sq")}
+                   "lamb": ("exp_avg", "exp_avg_sq"), "lars": ("momentum_buffer",)}
 
     def state_dict(self):
         """The optimizer state in ``torch.optim``'s format.
@@ -398,15 +402,16 @@ class _DistributedOptimizer(torch.optim.Optimizer):
                 ent = full.get(p)
                 if ent is not None:
                     e = {}
-                    if t > 0 and self._fused == "sgd":
-                        if g.get("momentum", 0) != 0:
+                    if t > 0 and self._fused in ("sgd", "lars"):
+                        # Lars keeps its buffer whatever the momentum, as the plain optimizer does
+                        if self._fused == "lars" or g.get("momentum", 0) != 0:
                             e["momentum_buffer"] = ent["state0"]
                     elif t > 0:
                         e["step"] = torch.tensor(float(t), dtype=torch.float32)
                         e["exp_avg"], e["exp_avg_sq"] = ent["state0"], ent["state1"]
                     # torch's Adam creates its state only for a parameter without any: an entry holding only the
                     # masters (nothing has been stepped yet, so they equal the weights) would stop it
-                    if p.dtype != torch.float32 and (t > 0 or self._fused == "sgd"):
+                    if p.dtype != torch.float32 and (t > 0 or self._fused in ("sgd", "lars")):
                         e["master_param"] = ent["master"]
                     if e:
                         state[idx] = e
@@ -429,7 +434,8 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         earlier stay valid) and the full tensors are also kept in ``self.state`` until
         ``broadcast_optimizer_state`` hands them to the other ranks, so loading on rank 0 only works.  The next
         ``step()`` (or ``refresh_hparams()`` before a graph replay) drops them if no broadcast came first.  A
-        ``momentum_buffer`` means SGD has taken a step; Adam's ``step`` must be equal within a param group.
+        ``momentum_buffer`` means SGD or Lars has taken a step; Adam's ``step`` must be equal within a param group.
+        A Lars buffer includes the learning rate, so it does not move between Lars and ``torch.optim.SGD``.
         Missing entries start fresh: master weights from the current parameters (load the model first),
         zero moments.
         """
@@ -450,7 +456,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         steps = []
         for g in self.param_groups:
             ents = [full[p] for p in g["params"] if p in full]
-            if self._fused == "sgd":
+            if self._fused in ("sgd", "lars"):
                 steps.append(1 if any("momentum_buffer" in e for e in ents) else 0)
                 continue
             vals = sorted({float(e["step"]) for e in ents if "step" in e})
@@ -485,7 +491,7 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
 
     Arguments match the reference (optimizer, named_parameters, compression,
     backward_passes_per_step).  Extras: ``fused_update=True`` applies the
-    SGD, Adam(W) or :class:`Lamb` step on fp32 master weights inside the
+    SGD, Adam(W), :class:`Lamb` or :class:`Lars` step on fp32 master weights inside the
     exchange kernels;
     ``bucket_bytes`` sets the fusion granularity; ``compression_params`` (e.g.
     ``{"compressor": "topk", "k": 0.01, "ef": "vanilla"}``, docs/gradient-compression.md)

@@ -31,7 +31,11 @@ p.add_argument("--warmup-epochs", type=float, default=1)
 p.add_argument("--model", default="resnet50")
 p.add_argument("--image-size", type=int, default=224)
 p.add_argument("--no-cuda", action="store_true")
-p.add_argument("--fused-update", action="store_true", help="SGD step inside the exchange kernel (fp32 master shards)")
+p.add_argument("--fused-update", action="store_true",
+               help="optimizer step inside the exchange kernels (fp32 master shards)")
+p.add_argument("--optimizer", choices=("sgd", "lars"), default="sgd",
+               help="lars: byteps_b200.torch.Lars, with batch-norm parameters and biases in an adapt=False, "
+                    "weight_decay=0 group")
 p.add_argument("--sync-bn", action="store_true",
                help="batch-norm statistics over all ranks' batches (bps.convert_sync_batchnorm; CUDA channels_last)")
 args = p.parse_args()
@@ -50,8 +54,15 @@ model = get_model(args.model).to(dev)
 if args.sync_bn:
     # synchronised training takes NHWC (channels_last) activations; converting is collective
     model = bps.convert_sync_batchnorm(model.to(memory_format=torch.channels_last))
-opt = torch.optim.SGD(model.parameters(), lr=args.base_lr * args.batches_per_pushpull * bps.size(), momentum=0.9,
-                      weight_decay=5e-5)
+lr = args.base_lr * args.batches_per_pushpull * bps.size()
+if args.optimizer == "lars":
+    # the large-batch recipe: no trust ratio and no decay for batch-norm parameters and biases (1-d tensors)
+    decayed = [q for q in model.parameters() if q.dim() > 1]
+    plain = [q for q in model.parameters() if q.dim() <= 1]
+    opt = bps.Lars([dict(params=decayed, weight_decay=5e-5), dict(params=plain, weight_decay=0.0, adapt=False)],
+                   lr=lr, momentum=0.9)
+else:
+    opt = torch.optim.SGD(model.parameters(), lr=lr, momentum=0.9, weight_decay=5e-5)
 opt = bps.DistributedOptimizer(opt, named_parameters=model.named_parameters(),
                                backward_passes_per_step=args.batches_per_pushpull,
                                fused_update=args.fused_update and cuda)
