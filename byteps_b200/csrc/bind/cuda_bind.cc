@@ -250,4 +250,5 @@ PYBIND11_MODULE(_cuda, m) {
   bind_cuda_fp8(m);
   bind_cuda_lamb(m);
   bind_cuda_lars(m);
+  bind_cuda_clip(m);
 }

@@ -12,3 +12,4 @@ void bind_cuda_xent(pybind11::module_& m);
 void bind_cuda_fp8(pybind11::module_& m);
 void bind_cuda_lamb(pybind11::module_& m);
 void bind_cuda_lars(pybind11::module_& m);
+void bind_cuda_clip(pybind11::module_& m);

@@ -111,7 +111,8 @@ class Bucket:
     ring_cls: Optional[tuple] = None                   # (wire code, ring kind) of the ring table it belongs to
     ring_pos: int = -1                                 # position inside that table
     lamb_win_off: int = -1                             # byte offset of the norm window (fused LAMB and LARS)
-    lamb_params: Optional[torch.Tensor] = None         # LAMB, LARS: (start, numel) per parameter, int64 on the device
+    lamb_params: Optional[torch.Tensor] = None         # LAMB, LARS, clipping: (start, numel) per parameter, int64
+    normed: bool = False                               # clipping: this step's norm pass has been issued
 
     @property
     def nbytes(self) -> int:
@@ -140,15 +141,21 @@ class BucketedGradSync:
 
     def __init__(self, engine, param_groups, *, fused: Optional[str] = None, wire_dtype: Optional[torch.dtype] = None,
                  bucket_bytes: Optional[int] = None, backward_passes_per_step: int = 1, average: bool = True,
-                 priority_of: Optional[Dict] = None, loss_scaler: Optional[Dict] = None):
+                 priority_of: Optional[Dict] = None, loss_scaler: Optional[Dict] = None,
+                 max_grad_norm: Optional[float] = None):
         """loss_scaler (fused mode only): dynamic loss scaling on the device, a dict with GradScaler's
-        init_scale, growth_factor, backoff_factor and growth_interval (see `_issue_scaled_step`)."""
+        init_scale, growth_factor, backoff_factor and growth_interval (see `_issue_deferred_step`).
+        max_grad_norm (fused mode only): clip the averaged gradients by their global 2-norm before the update, as
+        torch.nn.utils.clip_grad_norm_ does (see `_issue_deferred_step`)."""
         self.engine = engine
         self.world, self.rank = engine.size, engine.rank
         self.fused = fused                     # None | "sgd" | "adam" | "adamw" | "lamb" | "lars"
         if loss_scaler is not None and not fused:
             raise ValueError("dynamic loss scaling needs the fused optimizer")
         self.loss_scaler = dict(loss_scaler) if loss_scaler is not None else None
+        if max_grad_norm is not None and not fused:
+            raise ValueError("max_grad_norm in the exchange needs the fused optimizer")
+        self.max_grad_norm = max_grad_norm
         reduce_engine = os.environ.get("BYTEPS_REDUCE_ENGINE", "auto").lower()
         if reduce_engine not in REDUCE_ENGINES:
             raise ValueError("BYTEPS_REDUCE_ENGINE=%s: expected one of %s (the tensor-core engine of sm_90a is 'wgmma')"
@@ -207,6 +214,11 @@ class BucketedGradSync:
             # the overflow flags every rank publishes to every peer (loss_scale_update), only in this mode
             self.ls_win_off = off
             off += 256
+        self.clip_win_off = -1
+        if max_grad_norm is not None:
+            # every rank's float64 sum of squares, published to every peer (clip_norm_update), only in this mode
+            self.clip_win_off = off
+            off += 256
         cfg = engine.cfg
         stamp("buckets: layout of %d buckets, arena %d MiB" % (len(self.buckets), off >> 20))
         self.ctx = SymmContext(engine.group, self.device, max(off, 4096), cfg.symm_mode, cfg.use_nvls)
@@ -239,6 +251,8 @@ class BucketedGradSync:
             self._init_fused_state()
         if self.loss_scaler is not None:
             self._init_loss_scaler()
+        if max_grad_norm is not None:
+            self._init_clip()
         self._next = 0          # strict mode: next bucket index allowed to launch
         self._strict = os.environ.get("BYTEPS_STRICT_ORDER", "0") not in ("0", "")
         self._hooks = []
@@ -324,14 +338,20 @@ class BucketedGradSync:
             cu.lamb_load_kernels()
         else:
             cu.lars_load_kernels()
-        for b in self.buckets:
-            b.lamb_params = torch.tensor([[st, p.numel()] for p, st in zip(b.params, b.starts)], dtype=torch.int64,
-                                         device=self.device)
+        self._build_param_tables()
         nmax = max(len(b.params) for b in self.buckets)
         shard_max = max(s1 - s0 for s0, s1 in map(self.shard_range, self.buckets))
         self._lamb_scratch = torch.zeros(cu.lamb_scratch_bytes(shard_max, nmax) // 8, dtype=torch.float64,
                                          device=self.device)
         self._lamb_phi = torch.ones(nmax, dtype=torch.float32, device=self.device)
+
+    def _build_param_tables(self):
+        """Every bucket's (start, numel) table on the device: the parameter cursor of the norm kernels keeps padding
+        out of every norm with it."""
+        for b in self.buckets:
+            if b.lamb_params is None:
+                b.lamb_params = torch.tensor([[st, p.numel()] for p, st in zip(b.params, b.starts)],
+                                             dtype=torch.int64, device=self.device)
 
     def lamb_device_bytes(self) -> int:
         """Device bytes fused LAMB adds to fused Adam, or fused LARS to fused SGD, on this rank: tables, scratch,
@@ -341,6 +361,54 @@ class BucketedGradSync:
         windows = sum(self.ctx.cu.lamb_window_bytes(len(b.params), self.world) for b in self.buckets)
         return (sum(b.lamb_params.nbytes for b in self.buckets) + self._lamb_scratch.nbytes + self._lamb_phi.nbytes
                 + windows)
+
+    # ------------------------------------------------------------------ gradient clipping (fused mode)
+    def _init_clip(self):
+        """Device state of global gradient-norm clipping: the (start, numel) tables, one float64 scratch row per bucket
+        (one entry per CTA of its norm pass; entries no CTA writes stay zero and add nothing), the total norm and
+        the agreement window."""
+        cu = self.ctx.cu
+        cu.clip_load_kernels()           # loaded before any launch that spins on a peer (DESIGN 1.6)
+        self._build_param_tables()
+        row = max(self._blocks(b) for b in self.buckets)
+        self._clip_scratch = torch.zeros((len(self.buckets), row), dtype=torch.float64, device=self.device)
+        self._grad_norm = torch.zeros((), dtype=torch.float32, device=self.device)
+        self.ctx.tensor(self.clip_win_off, 256, torch.uint8).zero_()
+
+    def grad_norm_tensor(self) -> torch.Tensor:
+        """0-dim float32 device tensor: the last step's total gradient norm before clipping, written by the kernels
+        (so also by every replay of a captured step)."""
+        return self._grad_norm
+
+    def clip_device_bytes(self) -> int:
+        """Device bytes clipping adds on this rank: the (start, numel) tables (unless LAMB or LARS has them anyway),
+        the scratch rows, the total norm and the agreement window."""
+        if self.max_grad_norm is None:
+            return 0
+        tables = 0 if self.fused in _TRUST_KINDS else sum(b.lamb_params.nbytes for b in self.buckets)
+        return tables + self._clip_scratch.nbytes + self._grad_norm.nbytes + self.ctx.cu.CLIP_WINDOW_BYTES
+
+    def _launch_norm(self, b: Bucket, wait: bool = True):
+        """The norm pass of bucket b on the comm stream (clip_norm_partial): this rank's shard of the reduced gradient,
+        one float64 sum of squares per CTA into the bucket's scratch row."""
+        cu = self.ctx.cu
+        cs = self.comm_stream
+        if wait:
+            ev = torch.cuda.Event()
+            ev.record(torch.cuda.current_stream(self.device))
+            cs.wait_event(ev)
+        wire = self._wire(b)
+        if wire == b.dtype:
+            segs, nsegs, stage = 0, 0, b.grad_off
+        else:
+            segs, nsegs, stage = self._seg_table(b).data_ptr(), 1, self.stage_off
+        scale = (1.0 / self.world) if self.average else 1.0
+        row = self._clip_scratch[b.index].data_ptr()
+        cu.clip_norm_partial(self.ctx.view, wire_code(b.dtype), wire_code(wire), segs, nsegs, stage, b.numel, scale,
+                             b.lamb_params.data_ptr(), len(b.params), row, self._hp_dev.data_ptr() + 64 * b.group_index,
+                             self._blocks(b), self.threads, 0, self._nvls_for(wire), cs.cuda_stream)
+        b.normed = True
+        self._count_launch()
 
     # ------------------------------------------------------------------ dynamic loss scaling (fused mode)
     def _init_loss_scaler(self):
@@ -481,7 +549,10 @@ class BucketedGradSync:
             b = self._param_bucket[p]
             b.pending -= 1
             if b.pending == 0 and self.loss_scaler is None:   # dynamic loss scaling: launched at the step
-                self._launch_ready(b)
+                if self.max_grad_norm is None:
+                    self._launch_ready(b)
+                elif not self._strict:
+                    self._launch_norm(b)        # clipping: the norm pass now, the exchange at the step
         return hook
 
     def set_backward_passes_per_step(self, n: int):
@@ -527,6 +598,11 @@ class BucketedGradSync:
             self._seg_tables[b.index] = t
         return t
 
+    def _blocks(self, b: Bucket) -> int:
+        """CTAs of bucket b's exchange (and norm pass): a function of the bucket, the same on every rank."""
+        shard = (self._wire_bytes(b) + self.world - 1) // self.world
+        return self.engine.cfg.comm_blocks or pick_blocks(shard, self.threads, 32, cap=64)
+
     def _launch(self, b: Bucket):
         cu = self.ctx.cu
         view = self.ctx.view
@@ -544,9 +620,8 @@ class BucketedGradSync:
         wire = self._wire(b)
         world = self.world
         scale = (1.0 / world) if self.average else 1.0
-        wbytes = self._wire_bytes(b)
-        shard = (wbytes + world - 1) // world
-        blocks = self.engine.cfg.comm_blocks or pick_blocks(shard, self.threads, 32, cap=64)
+        shard = (self._wire_bytes(b) + world - 1) // world
+        blocks = self._blocks(b)
         nvls = self._nvls_for(wire)
         if self.fused in _TRUST_KINDS:
             self._launch_trust(b, wire, scale, blocks, nvls, cs)
@@ -680,8 +755,8 @@ class BucketedGradSync:
             mode = "batch" if (self.world > 1 and eligible) else "off"
         if mode != "off" and not eligible:
             mode = "off"
-        if mode == "persistent" and self.loss_scaler is not None:
-            mode = "batch"      # every exchange waits for the overflow decision at the step: nothing to start early
+        if mode == "persistent" and (self.loss_scaler is not None or self.max_grad_norm is not None):
+            mode = "batch"      # every exchange waits for a decision at the step (overflow, norm): nothing to start early
         self._ring_mode = mode
         if mode == "off":
             return
@@ -876,8 +951,8 @@ class BucketedGradSync:
 
     def _issue_remaining(self):
         """Issue every bucket that has not gone out yet (unused parameters), in index order on every rank."""
-        if self.loss_scaler is not None:
-            self._issue_scaled_step()
+        if self.loss_scaler is not None or self.max_grad_norm is not None:
+            self._issue_deferred_step()
             return
         for b in self.buckets:
             if not b.launched:
@@ -886,16 +961,23 @@ class BucketedGradSync:
                 self._issue(b)
         self._ring_flush()
 
-    def _issue_scaled_step(self):
-        """Dynamic loss scaling: the whole exchange of the step, issued at the step on the comm stream.
+    def _issue_deferred_step(self):
+        """Dynamic loss scaling and gradient clipping: the exchanges of the step, issued at the step on the comm
+        stream, after a decision every rank takes on the device.
 
-        1. loss_scale_check: does any element of this rank's gradient windows overflow on its wire?
-        2. loss_scale_update: every rank learns every rank's flag (barrier_peers, OR in rank order), updates the
-           scale, counts the step per group if it is applied, and writes grad_scale = 1/S, skip, first_step and the
-           Adam bias corrections into the hyper-parameter blocks, over what refresh_hparams put there.
+        1. dynamic loss scaling: loss_scale_check (does any element of this rank's gradient windows overflow on its
+           wire?) and loss_scale_update (every rank learns every rank's flag by barrier_peers and an OR in rank
+           order, updates the scale, counts the step per group if it is applied, and writes grad_scale = 1/S, skip,
+           first_step and the Adam bias corrections into the hyper-parameter blocks, over what refresh_hparams put
+           there).
+        2. clipping: clip_norm_partial for every bucket whose hook has not launched it during backward (all of them
+           with loss scaling, which must unscale first), in bucket order; then clip_norm_update, which sums the
+           squares over every bucket and rank, writes the norm and multiplies every group's grad_scale by
+           min(1, max_grad_norm / (norm + 1e-6)).  grad_scale is rewritten before every step (refresh_hparams,
+           pre_replay or loss_scale_update), so the coefficient never compounds.
         3. every bucket's fused exchange in bucket order: one ring flush (BYTEPS_RING=batch, and persistent, which
            behaves as batch here) or one launch per bucket; a skipped step leaves the optimizer state as it is.
-        The hooks launched nothing during backward, so the update no longer overlaps with it."""
+        No exchange went out during backward, so the update no longer overlaps with it."""
         for b in self.buckets:
             if not b.launched:
                 self._zero_unused(b)
@@ -906,13 +988,22 @@ class BucketedGradSync:
         ev = torch.cuda.Event()
         ev.record(cur)
         cs.wait_event(ev)
-        state = self._ls_state.data_ptr()
-        cu.loss_scale_check(self.ctx.view, self._ls_table.data_ptr(), len(self.buckets), self._ls_max_vectors, state,
-                            cs.cuda_stream)
-        cu.loss_scale_update(self.ctx.view, 0, self.ls_win_off, state, self._ls_steps.data_ptr(),
-                             self._ls_betas.data_ptr(), self._hp_dev.data_ptr(), len(self.param_groups),
-                             self.fused not in ("sgd", "lars"), cs.cuda_stream)
-        self._count_launch(2)
+        if self.loss_scaler is not None:
+            state = self._ls_state.data_ptr()
+            cu.loss_scale_check(self.ctx.view, self._ls_table.data_ptr(), len(self.buckets), self._ls_max_vectors,
+                                state, cs.cuda_stream)
+            cu.loss_scale_update(self.ctx.view, 0, self.ls_win_off, state, self._ls_steps.data_ptr(),
+                                 self._ls_betas.data_ptr(), self._hp_dev.data_ptr(), len(self.param_groups),
+                                 self.fused not in ("sgd", "lars"), cs.cuda_stream)
+            self._count_launch(2)
+        if self.max_grad_norm is not None:
+            for b in self.buckets:
+                if not b.normed:
+                    self._launch_norm(b, wait=False)
+            cu.clip_norm_update(self.ctx.view, 0, self.clip_win_off, self._clip_scratch.data_ptr(), len(self.buckets),
+                                self._clip_scratch.shape[1], float(self.max_grad_norm), self._grad_norm.data_ptr(),
+                                self._hp_dev.data_ptr(), len(self.param_groups), cs.cuda_stream)
+            self._count_launch()
         for b in self.buckets:
             if self._ring_mode != "off" and b.ring_cls is not None:
                 self._ring_pending.append(b)
@@ -994,6 +1085,7 @@ class BucketedGradSync:
         for b in self.buckets:
             b.pending = len(b.params)
             b.launched = False
+            b.normed = False
         for p in self._delay:
             self._delay[p] = self.bpps
 

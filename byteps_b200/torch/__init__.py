@@ -90,6 +90,21 @@ def _loss_scale_config(option):
         "dynamic_loss_scale", cfg["init_scale"], cfg["growth_factor"], cfg["backoff_factor"], cfg["growth_interval"])))
 
 
+def _checked_max_grad_norm(value):
+    """max_grad_norm as a float, or ValueError: None (no clipping) or a finite number > 0."""
+    if value is None:
+        return None
+    if isinstance(value, bool):
+        raise ValueError("max_grad_norm must be a finite number > 0, got %r" % (value,))
+    try:
+        v = float(value)
+    except (TypeError, ValueError):
+        raise ValueError("max_grad_norm must be a finite number > 0, got %r" % (value,)) from None
+    if not (math.isfinite(v) and v > 0):
+        raise ValueError("max_grad_norm must be a finite number > 0, got %r" % (value,))
+    return v
+
+
 def _checked_scaler_entry(ls):
     """A loaded "loss_scaler" entry (GradScaler.state_dict()'s keys) as (scale, growth_factor, backoff_factor,
     growth_interval, growth_tracker), checked like the constructor's options, or ValueError."""
@@ -123,11 +138,12 @@ def _checked_scaler_values(what, scale, growth, backoff, interval):
 
 class _DistributedOptimizer(torch.optim.Optimizer):
     def __init__(self, params, named_parameters, compression, backward_passes_per_step=1, fused_update=None,
-                 bucket_bytes=None, compression_params=None, dynamic_loss_scale=None):
+                 bucket_bytes=None, compression_params=None, dynamic_loss_scale=None, max_grad_norm=None):
         super(self.__class__, self).__init__(params)
         if fused_update is None:
             fused_update = os.getenv("BYTEPS_FUSED_OPTIMIZER", "0") not in ("0", "")
         loss_scaler = _loss_scale_config(dynamic_loss_scale)
+        self._max_grad_norm = _checked_max_grad_norm(max_grad_norm)
         if loss_scaler is not None and not fused_update:
             raise ValueError("dynamic_loss_scale needs fused_update=True")
         self._compression = compression
@@ -139,6 +155,8 @@ class _DistributedOptimizer(torch.optim.Optimizer):
         self._async_seeded = False
         if self._enable_async:
             assert int(os.getenv('DMLC_NUM_WORKER', 1)) > 1, "Async is only valid for distributed training"
+            if self._max_grad_norm is not None:
+                raise ValueError("max_grad_norm clips the averaged gradients; BYTEPS_ENABLE_ASYNC never averages them")
         if any(not isinstance(p, tuple) for p in named_parameters):
             raise ValueError('named_parameters should be a sequence of tuples (name, parameter), '
                              'usually produced by model.named_parameters().')
@@ -194,13 +212,17 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             self._sync = BucketedGradSync(eng, self.param_groups, fused=kind, wire_dtype=_wire_of(compression),
                                           bucket_bytes=bucket_bytes,
                                           backward_passes_per_step=backward_passes_per_step,
-                                          priority_of=self._priority, loss_scaler=loss_scaler)
+                                          priority_of=self._priority, loss_scaler=loss_scaler,
+                                          max_grad_norm=self._max_grad_norm if kind else None)
             if kind:
                 self._sync.refresh_hparams()
         elif size() > 1 or eng.backend == "ps":
             # one worker behind a server (BYTEPS_FORCE_DISTRIBUTED=1, the reference's test harness) still goes
             # through the servers: that is what applies the two compression stages
             self._register_hooks()
+        if self._max_grad_norm is not None and not self._fused:
+            # the unfused paths clip with torch itself and keep its result here
+            self._grad_norm = torch.zeros((), dtype=torch.float32, device=all_params[0].device)
 
     @staticmethod
     def find_duplicates(lst):
@@ -337,11 +359,24 @@ class _DistributedOptimizer(torch.optim.Optimizer):
             set_learning_rate(self.param_groups[0]["lr"])     # error feedback rescales by lr_prev/lr
         if self._should_sync:
             self.synchronize()
+        if self._max_grad_norm is not None:
+            params = [p for g in self.param_groups for p in g["params"]]
+            self._grad_norm.copy_(torch.nn.utils.clip_grad_norm_(params, self._max_grad_norm))
         return super(self.__class__, self).step(closure)
 
     @property
     def grad_sync(self):
         return self._sync
+
+    @property
+    def grad_norm(self):
+        """The last step's total gradient norm before clipping, as ``clip_grad_norm_`` returns it: a 0-dim float32
+        tensor.  With ``fused_update=True`` it is a device tensor the kernels write (a captured step updates it on
+        every replay); reading it does not synchronise, ``.item()`` does.  On a step dynamic loss scaling skipped it
+        holds the non-finite norm that was computed."""
+        if self._max_grad_norm is None:
+            raise RuntimeError("this optimizer was built without max_grad_norm")
+        return self._sync.grad_norm_tensor() if self._fused else self._grad_norm
 
     # ---- dynamic loss scaling (fused mode) ------------------------------------------
     def _scaler(self):
@@ -485,7 +520,7 @@ class _DistributedOptimizer(torch.optim.Optimizer):
 
 def DistributedOptimizer(optimizer, named_parameters=None, compression=Compression.none,
                          backward_passes_per_step=1, fused_update=None, bucket_bytes=None, compression_params=None,
-                         dynamic_loss_scale=False):
+                         dynamic_loss_scale=False, max_grad_norm=None):
     """Wrap ``optimizer`` so gradients are averaged over all processes before
     ``step()``; communication overlaps with ``loss.backward()``.
 
@@ -498,8 +533,18 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
     turns on lossy gradient compression per tensor - GPU kernels over NVLink, or the
     worker/server compressors in CPU-server mode.
 
-    ``synchronize()`` forces completion (e.g. before gradient clipping),
-    ``skip_synchronize()`` lets a following ``step()`` skip it.
+    ``synchronize()`` forces completion, ``skip_synchronize()`` lets a following ``step()`` skip it.
+
+    ``max_grad_norm`` (a finite float > 0): clip the gradients by their global 2-norm before every update, with
+    ``torch.nn.utils.clip_grad_norm_``'s rule.  The norm N is taken over every parameter of every param group, on
+    the averaged gradient (with ``dynamic_loss_scale``, the unscaled one), and the update runs on
+    ``min(1, max_grad_norm / (N + 1e-6)) * g``.  Only the 2-norm is supported.  ``grad_norm`` holds N of the last
+    step.  With ``fused_update=True`` the norm is taken and applied inside the exchange on the device, with no host
+    synchronisation, so the step still captures into a CUDA graph; the exchanges then wait for the last gradient,
+    so the update no longer overlaps with backward.  Every other configuration runs ``synchronize()``,
+    ``clip_grad_norm_`` over all parameters and the wrapped ``step()``.  With ``fused_update=True``, a
+    ``clip_grad_norm_`` of your own between ``synchronize()`` and ``step()`` has no effect: the update has already
+    happened, and ``.grad`` holds this rank's unreduced gradients.
 
     ``dynamic_loss_scale`` (with ``fused_update=True``, symmetric-memory or local backend): dynamic loss scaling
     for fp16 training, decided on the device.  ``True`` uses ``torch.amp.GradScaler``'s defaults; a dict overrides
@@ -513,7 +558,7 @@ def DistributedOptimizer(optimizer, named_parameters=None, compression=Compressi
     """
     cls = type(optimizer.__class__.__name__, (optimizer.__class__,), dict(_DistributedOptimizer.__dict__))
     return cls(optimizer.param_groups, named_parameters, compression, backward_passes_per_step, fused_update,
-               bucket_bytes, compression_params, dynamic_loss_scale)
+               bucket_bytes, compression_params, dynamic_loss_scale, max_grad_norm)
 
 
 def broadcast_parameters(params, root_rank, prefix="Parameter."):

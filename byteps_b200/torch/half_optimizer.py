@@ -22,7 +22,8 @@ class HalfPrecisionDistributedOptimizer:
     inspected, so the exchange and the update are separate - gradients are averaged by the bucketed
     (or per-parameter) exchange, checked for inf/nan, unscaled into fp32 master gradients, the wrapped
     optimizer steps on fp32 MASTER copies and the half-precision weights are refreshed from them; the
-    scale halves on overflow (step skipped) and doubles after ``scale_window`` clean steps."""
+    scale halves on overflow (step skipped) and doubles after ``scale_window`` clean steps.
+    Global gradient-norm clipping (``DistributedOptimizer``'s ``max_grad_norm``) is not offered here."""
 
     def __init__(self, optimizer, named_parameters=None, loss_scale: float = 1.0, dynamic_loss_scale: bool = False,
                  scale_window: int = 1000, bucket_bytes=None):

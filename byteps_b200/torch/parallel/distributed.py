@@ -8,6 +8,7 @@ are exchanged by the zero-copy bucketed kernels
 (:class:`byteps_b200.parallel.bucket.BucketedGradSync`); elsewhere by
 per-parameter ``push_pull_group_sync_inplace`` like the reference, whose grad
 counter tells the wrapper when the last gradient of the iteration was issued.
+Clipping inside the exchange (``DistributedOptimizer``'s ``max_grad_norm``) is not offered by this wrapper.
 """
 from contextlib import contextmanager
 

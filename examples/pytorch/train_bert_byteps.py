@@ -28,6 +28,8 @@ p.add_argument("--fp8-linear", action="store_true",
                help="FP8 GEMMs with delayed scaling for the encoder layers' linear layers (sm_90)")
 p.add_argument("--optimizer", choices=("adamw", "lamb"), default="adamw",
                help="lamb: weights with decay and the trust ratio; biases and LayerNorm weights without either")
+p.add_argument("--max-grad-norm", type=float, default=None,
+               help="clip the averaged gradients by their global 2-norm before every update (BERT recipes use 1.0)")
 args = p.parse_args()
 bps.init()
 cuda = torch.cuda.is_available() and not args.no_cuda
@@ -46,7 +48,8 @@ if args.optimizer == "lamb":
                       dict(params=plain, weight_decay=0.0, adapt=False)], lr=1e-3)
 else:
     inner = torch.optim.AdamW(model.parameters(), lr=1e-4, weight_decay=0.01)
-opt = bps.DistributedOptimizer(inner, named_parameters=model.named_parameters(), fused_update=cuda)
+opt = bps.DistributedOptimizer(inner, named_parameters=model.named_parameters(), fused_update=cuda,
+                               max_grad_norm=args.max_grad_norm)
 bps.broadcast_parameters(model.state_dict(), root_rank=0)
 ids = torch.randint(0, 30522, (args.batch_size, args.seq_len), device=dev)
 labels = torch.randint(0, 30522, (args.batch_size, args.seq_len), device=dev)
