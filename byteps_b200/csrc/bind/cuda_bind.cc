@@ -251,4 +251,5 @@ PYBIND11_MODULE(_cuda, m) {
   bind_cuda_lamb(m);
   bind_cuda_lars(m);
   bind_cuda_clip(m);
+  bind_cuda_attn(m);
 }

@@ -228,6 +228,36 @@ struct TagF16 {
   __device__ static Vec16 mm_reduce(const void* mc) { return mm_ld_reduce_f16x8(mc); }
 };
 
+// ---- dropout bits ---------------------------------------------------------------
+// Philox4x32-10 with counter c and key k.  Dropout keeps element i when word i % 4 of the Philox block with counter
+// (i / 4, offset) and key seed is below keep = (1 - p) * 2^32; the LayerNorm and attention kernels share the scheme.
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+  for (int i = 0; i < 10; ++i) {
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+    k.x += 0x9E3779B9u;
+    k.y += 0xBB67AE85u;
+  }
+  return c;
+}
+
+// the 4 keep bits of Philox block (counter g, offset off): bit j for element 4g + j
+__device__ __forceinline__ uint32_t keep_nibble(uint2 key, uint2 off, uint64_t g, uint32_t keep) {
+  const uint4 r = philox4x32_10(make_uint4((uint32_t)g, (uint32_t)(g >> 32), off.x, off.y), key);
+  return (uint32_t)(r.x < keep) | (uint32_t)(r.y < keep) << 1 | (uint32_t)(r.z < keep) << 2 |
+         (uint32_t)(r.w < keep) << 3;
+}
+
+// keep bits of the 8 elements from element index e (a multiple of 4): bit k for element e + k
+__device__ __forceinline__ uint32_t keep_bits(uint2 key, uint2 off, uint64_t e, uint32_t keep) {
+  uint32_t bits = 0;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) bits |= keep_nibble(key, off, (e >> 2) + h, keep) << (4 * h);
+  return bits;
+}
+
 }  // namespace bps
 
 // ---- mbarrier + bulk async copy (TMA, 1-D form: no tensor map needed) -------------------------

@@ -51,31 +51,6 @@ struct Io {
   }
 };
 
-__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
-#pragma unroll
-  for (int i = 0; i < 10; ++i) {
-    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
-    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
-    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
-    k.x += 0x9E3779B9u;
-    k.y += 0xBB67AE85u;
-  }
-  return c;
-}
-
-// keep bits of the 8 elements from element index e (a multiple of 4): bit k for element e + k
-__device__ __forceinline__ uint32_t keep_bits(uint2 key, uint2 off, uint64_t e, uint32_t keep) {
-  uint32_t bits = 0;
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const uint64_t c = (e >> 2) + h;
-    const uint4 r = philox4x32_10(make_uint4((uint32_t)c, (uint32_t)(c >> 32), off.x, off.y), key);
-    bits |= ((uint32_t)(r.x < keep) | (uint32_t)(r.y < keep) << 1 | (uint32_t)(r.z < keep) << 2 |
-             (uint32_t)(r.w < keep) << 3) << (4 * h);
-  }
-  return bits;
-}
-
 // Sum of the K values over the TPR threads of row group `grp`, returned to all of them.  Wider groups go through
 // sh[K][TPR / 32]; callers alternate between two such buffers, so a buffer is written again only after every thread
 // of the group has passed the barrier of the reduction in between.

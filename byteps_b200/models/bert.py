@@ -8,6 +8,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from ..ops.attn import self_attention
 from ..ops.fp8 import Fp8Linear, fp8_gelu_mlp
 from ..ops.ln import DropoutAddLayerNorm
 from ..ops.xent import softmax_cross_entropy
@@ -34,6 +35,10 @@ class BertConfig:
     # (same parameters and state_dict as nn.Linear); the heads stay in the model's dtype.  The GELU between fc1 and
     # fc2 then runs inside the FP8 casts (ops.fp8.fp8_gelu_mlp), with the same results
     fp8_linear: bool = False
+    # self-attention through ops.attn.self_attention: one fused kernel forward and two backward on CUDA read Q, K and
+    # V in place from the qkv projection and write the context and d(qkv) in the layouts the linears use (same
+    # parameters and state_dict; other inputs run the stock SDPA expression)
+    fused_attention: bool = False
 
 
 class BertEmbeddings(nn.Module):
@@ -72,12 +77,16 @@ class BertLayer(nn.Module):
         self.norm2 = _junction_norm(c)
         self.p = c.dropout
         self.fused_norm = c.fused_norm
+        self.fused_attention = c.fused_attention
 
     def forward(self, x, mask=None):
         b, s, e = x.shape
-        q, k, v = self.qkv(x).view(b, s, 3, self.h, self.d).permute(2, 0, 3, 1, 4)
-        a = F.scaled_dot_product_attention(q, k, v, attn_mask=mask, dropout_p=self.p if self.training else 0.0)
-        a = a.transpose(1, 2).reshape(b, s, e)
+        if self.fused_attention:
+            a = self_attention(self.qkv(x), self.h, mask, self.p, self.training)
+        else:
+            q, k, v = self.qkv(x).view(b, s, 3, self.h, self.d).permute(2, 0, 3, 1, 4)
+            a = F.scaled_dot_product_attention(q, k, v, attn_mask=mask, dropout_p=self.p if self.training else 0.0)
+            a = a.transpose(1, 2).reshape(b, s, e)
         if self.fused_norm:
             x = self.norm1(self.proj(a), x)
             return self.norm2(self.mlp(x), x)

@@ -22,6 +22,8 @@ p.add_argument("--warmup-steps", type=int, default=5)
 p.add_argument("--no-cuda", action="store_true", help="CPU run over gloo (unfused optimizer, fp32)")
 p.add_argument("--fused-norm", action="store_true",
                help="fused dropout + residual add + LayerNorm kernels at the encoder layers' junctions")
+p.add_argument("--fused-attention", action="store_true",
+               help="fused self-attention kernels reading Q, K and V in place from the qkv projection")
 p.add_argument("--fused-loss", action="store_true",
                help="fused softmax cross-entropy kernels for the masked-LM loss")
 p.add_argument("--fp8-linear", action="store_true",
@@ -37,7 +39,7 @@ if cuda:
     torch.cuda.set_device(bps.local_rank())
 dev = torch.device("cuda", bps.local_rank()) if cuda else torch.device("cpu")
 model = get_model(args.model, fused_norm=args.fused_norm, fused_loss=args.fused_loss,
-                  fp8_linear=args.fp8_linear).to(dev)
+                  fp8_linear=args.fp8_linear, fused_attention=args.fused_attention).to(dev)
 if cuda:
     model = model.to(torch.bfloat16)
 if args.optimizer == "lamb":
