@@ -2,6 +2,7 @@
 #include <cuda_runtime_api.h>
 #include <pybind11/pybind11.h>
 
+#include <initializer_list>
 #include <stdexcept>
 #include <string>
 
@@ -27,6 +28,21 @@ void check_shape(int dtype, int B, int S, int H, int D, int mask_kind) {
     throw std::invalid_argument("attention: batch and heads must be in [1, 65535]");
   if (mask_kind < ATTN_MASK_F32 || mask_kind > ATTN_MASK_BOOL)
     throw std::invalid_argument("attention: unknown mask kind " + std::to_string(mask_kind));
+}
+
+void check_varlen(int dtype, int T, int N, int H, int D, int max_seqlen, uintptr_t cu) {
+  check_shape(dtype, 1, max_seqlen, H, D, ATTN_MASK_F32);
+  if (T < 1) throw std::invalid_argument("attention: token count must be >= 1, got " + std::to_string(T));
+  if (N < 1 || N > 65535)
+    throw std::invalid_argument("attention: sequence count must be in [1, 65535], got " + std::to_string(N));
+  if (cu == 0 || cu % 4 != 0) throw std::invalid_argument("attention: cu_seqlens must be a 4-byte aligned pointer");
+}
+
+void check_ptrs(std::initializer_list<uintptr_t> p16, std::initializer_list<uintptr_t> p4) {
+  for (uintptr_t p : p16)
+    if (p == 0 || p % 16 != 0) throw std::invalid_argument("attention: tensors must be non-null and 16-byte aligned");
+  for (uintptr_t p : p4)
+    if (p == 0 || p % 4 != 0) throw std::invalid_argument("attention: fp32 tensors must be non-null and aligned");
 }
 }  // namespace
 
@@ -61,4 +77,31 @@ void bind_cuda_attn(py::module_& m) {
      py::arg("H"), py::arg("D"), py::arg("mask"), py::arg("mask_kind"), py::arg("mask_bstride"), py::arg("seed"),
      py::arg("keep"), py::arg("scale"), py::arg("delta"), py::arg("dqkv"), py::arg("stream"),
      "dqkv [B, S, 3, H, 64] of attn_fwd's output given dout; delta: fp32 [B, H, S] workspace");
+
+  m.def("attn_varlen_fwd", [](uintptr_t qkv, int dtype, int T, int N, int H, int D, int max_seqlen,
+                              uintptr_t cu_seqlens, uintptr_t seed, uint32_t keep, float scale, uintptr_t out,
+                              uintptr_t lse, uintptr_t s) {
+    check_varlen(dtype, T, N, H, D, max_seqlen, cu_seqlens);
+    check_ptrs({qkv, out}, {lse});
+    chk(launch_attn_varlen_fwd((const void*)qkv, dtype, T, N, H, D, max_seqlen, (const int*)cu_seqlens,
+                               (const int64_t*)seed, keep, scale, (void*)out, (float*)lse, (cudaStream_t)s),
+        "attn_varlen_fwd");
+  }, py::arg("qkv"), py::arg("dtype"), py::arg("T"), py::arg("N"), py::arg("H"), py::arg("D"),
+     py::arg("max_seqlen"), py::arg("cu_seqlens"), py::arg("seed"), py::arg("keep"), py::arg("scale"),
+     py::arg("out"), py::arg("lse"), py::arg("stream"),
+     "out [T, E] = attention of qkv [T, 3, H, 64] within the N sequences of device int32 cu_seqlens [N + 1], "
+     "each at most max_seqlen (<= 512) long; lse fp32 [H, T]; seed as for attn_fwd");
+  m.def("attn_varlen_bwd", [](uintptr_t qkv, uintptr_t out, uintptr_t dout, uintptr_t lse, int dtype, int T, int N,
+                              int H, int D, int max_seqlen, uintptr_t cu_seqlens, uintptr_t seed, uint32_t keep,
+                              float scale, uintptr_t delta, uintptr_t dqkv, uintptr_t s) {
+    check_varlen(dtype, T, N, H, D, max_seqlen, cu_seqlens);
+    check_ptrs({qkv, out, dout, dqkv}, {lse, delta});
+    chk(launch_attn_varlen_bwd((const void*)qkv, (const void*)out, (const void*)dout, (const float*)lse, dtype, T,
+                               N, H, D, max_seqlen, (const int*)cu_seqlens, (const int64_t*)seed, keep, scale,
+                               (float*)delta, (void*)dqkv, (cudaStream_t)s),
+        "attn_varlen_bwd");
+  }, py::arg("qkv"), py::arg("out"), py::arg("dout"), py::arg("lse"), py::arg("dtype"), py::arg("T"), py::arg("N"),
+     py::arg("H"), py::arg("D"), py::arg("max_seqlen"), py::arg("cu_seqlens"), py::arg("seed"), py::arg("keep"),
+     py::arg("scale"), py::arg("delta"), py::arg("dqkv"), py::arg("stream"),
+     "dqkv [T, 3, H, 64] of attn_varlen_fwd's output given dout; delta: fp32 [H, T] workspace");
 }

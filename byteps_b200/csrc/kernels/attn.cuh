@@ -20,6 +20,21 @@
 //
 // Every pointer but mask, lse and delta is 16-byte aligned.  Sums run in a fixed order and nothing is accumulated
 // with atomics, so results are bit-identical from run to run.
+//
+// Packed variable-length form (attn_varlen.cu): N sequences concatenated into one stream of T tokens, attention
+// never crossing a sequence boundary.
+//   qkv   [T, 3, H, 64], out / dout [T, E], dqkv like qkv, lse / delta fp32 [H, T]
+//   cu_seqlens  device int32 [N + 1]: sequence n is tokens [cu[n], cu[n + 1]); zero-length sequences are allowed, so
+//         a caller can pad the array to a fixed capacity by repeating its last value
+//   max_seqlen  host bound on every length, in [1, 512]; the grid is (ceil(max_seqlen / 64), H, N), fixed for a
+//         given capacity, so a launch captures into a CUDA graph and cu_seqlens may change between replays
+// Tokens outside every sequence (before cu[0], or from cu[N] on) get a zero context, lse = +inf and zero d(qkv).  A
+// sequence longer than max_seqlen gets NaN in its context, lse and d(qkv) rows.  Offsets are clamped into [0, T)
+// before any address is formed from them, so no cu_seqlens makes an access leave the buffers; for offsets out of
+// order the results are unspecified.
+// Dropout keeps element (head h, query token t, key token u of sequence n) when word i % 4 of the Philox block with
+// counter (i / 4, offset) is below `keep`, where i = (h T + t) * 512 + (u - cu[n]): the padded numbering with the
+// batch row replaced by the token and the key stride fixed at the longest supported sequence.
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -40,5 +55,13 @@ cudaError_t launch_attn_bwd(const void* qkv, const void* out, const void* dout, 
                             int S, int H, int D, const void* mask, int mask_kind, int64_t mask_bstride,
                             const int64_t* seed, uint32_t keep, float scale, float* delta, void* dqkv,
                             cudaStream_t s);
+
+cudaError_t launch_attn_varlen_fwd(const void* qkv, int dtype, int T, int N, int H, int D, int max_seqlen,
+                                   const int* cu_seqlens, const int64_t* seed, uint32_t keep, float scale, void* out,
+                                   float* lse, cudaStream_t s);
+cudaError_t launch_attn_varlen_bwd(const void* qkv, const void* out, const void* dout, const float* lse, int dtype,
+                                   int T, int N, int H, int D, int max_seqlen, const int* cu_seqlens,
+                                   const int64_t* seed, uint32_t keep, float scale, float* delta, void* dqkv,
+                                   cudaStream_t s);
 
 }  // namespace bps

@@ -8,7 +8,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from ..ops.attn import self_attention
+from ..ops.attn import _packed_tokens, _stock_varlen, self_attention
 from ..ops.fp8 import Fp8Linear, fp8_gelu_mlp
 from ..ops.ln import DropoutAddLayerNorm
 from ..ops.xent import softmax_cross_entropy
@@ -50,8 +50,9 @@ class BertEmbeddings(nn.Module):
         self.norm = nn.LayerNorm(c.hidden_size, eps=c.layer_norm_eps)
         self.drop = nn.Dropout(c.dropout)
 
-    def forward(self, ids, type_ids):
-        pos = torch.arange(ids.shape[1], device=ids.device).unsqueeze(0)
+    def forward(self, ids, type_ids, pos=None):
+        if pos is None:
+            pos = torch.arange(ids.shape[1], device=ids.device).unsqueeze(0)
         return self.drop(self.norm(self.word(ids) + self.pos(pos) + self.token_type(type_ids)))
 
 
@@ -79,10 +80,13 @@ class BertLayer(nn.Module):
         self.fused_norm = c.fused_norm
         self.fused_attention = c.fused_attention
 
-    def forward(self, x, mask=None):
+    def forward(self, x, mask=None, cu_seqlens=None, max_seqlen=None):
         b, s, e = x.shape
         if self.fused_attention:
-            a = self_attention(self.qkv(x), self.h, mask, self.p, self.training)
+            a = self_attention(self.qkv(x), self.h, mask, self.p, self.training, cu_seqlens=cu_seqlens,
+                               max_seqlen=max_seqlen)
+        elif cu_seqlens is not None:
+            a = _stock_varlen(self.qkv(x), self.h, cu_seqlens, max_seqlen, self.p if self.training else 0.0)
         else:
             q, k, v = self.qkv(x).view(b, s, 3, self.h, self.d).permute(2, 0, 3, 1, 4)
             a = F.scaled_dot_product_attention(q, k, v, attn_mask=mask, dropout_p=self.p if self.training else 0.0)
@@ -119,13 +123,33 @@ class BertForPreTraining(nn.Module):
             if isinstance(m, nn.Linear) and m.bias is not None:
                 nn.init.zeros_(m.bias)
 
-    def forward(self, ids, type_ids=None, mask=None, mlm_labels=None, nsp_labels=None):
+    def forward(self, ids, type_ids=None, mask=None, mlm_labels=None, nsp_labels=None, cu_seqlens=None,
+                max_seqlen=None):
+        """With ``cu_seqlens`` (device int32 [N + 1]), ``ids`` / ``type_ids`` / ``mlm_labels`` [B, S] are one packed
+        stream of T = B S tokens read row-major, in which sequence n is tokens [cu[n], cu[n + 1]); ``mask`` must be
+        None.  Token t takes position t - cu[n], NSP pools the first token of each sequence (``nsp_labels`` [N], -100
+        for empty slots), tokens outside every sequence take no MLM loss, and attention stays inside each sequence.
+        ``max_seqlen`` (default min(S, max_position)) bounds every length.  Nothing here reads cu_seqlens on the host,
+        so a step with fixed shapes captures into one CUDA graph."""
         if type_ids is None:
             type_ids = torch.zeros_like(ids)
-        x = self.embeddings(ids, type_ids)
+        pos = first = None
+        if cu_seqlens is not None:
+            if mask is not None:
+                raise ValueError("mask and cu_seqlens cannot be used together")
+            b, s = ids.shape
+            if max_seqlen is None:
+                max_seqlen = min(s, self.config.max_position)
+            t = torch.arange(b * s, device=ids.device)
+            seq, inside = _packed_tokens(cu_seqlens, t)
+            pos = (t - cu_seqlens[seq]).clamp(0, self.config.max_position - 1).view(b, s)
+            first = cu_seqlens[:-1].clamp(0, b * s - 1).long()
+            if mlm_labels is not None:
+                mlm_labels = mlm_labels.masked_fill(~inside.view(b, s), -100)
+        x = self.embeddings(ids, type_ids, pos)
         for layer in self.layers:
-            x = layer(x, mask)
-        pooled = torch.tanh(self.pooler(x[:, 0]))
+            x = layer(x, mask, cu_seqlens, max_seqlen)
+        pooled = torch.tanh(self.pooler(x[:, 0] if first is None else x.reshape(-1, x.shape[-1])[first]))
         h = self.mlm_norm(F.gelu(self.mlm_dense(x)))
         logits = F.linear(h, self.embeddings.word.weight, self.mlm_bias)   # tied decoder
         nsp_logits = self.nsp(pooled)
