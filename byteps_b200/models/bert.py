@@ -11,6 +11,7 @@ import torch.nn.functional as F
 from ..ops.attn import _packed_tokens, _stock_varlen, self_attention
 from ..ops.fp8 import Fp8Linear, fp8_gelu_mlp
 from ..ops.ln import DropoutAddLayerNorm
+from ..ops.mlm import gather_labelled
 from ..ops.xent import softmax_cross_entropy
 
 
@@ -39,6 +40,10 @@ class BertConfig:
     # V in place from the qkv projection and write the context and d(qkv) in the layouts the linears use (same
     # parameters and state_dict; other inputs run the stock SDPA expression)
     fused_attention: bool = False
+    # k > 0: with mlm_labels, the MLM head (dense, GELU, LayerNorm, tied decoder, loss) runs on the first C = B k
+    # labelled tokens of the batch only, gathered on the device by ops.mlm.gather_labelled, rather than on every token.
+    # Labelled tokens past C take no loss and are counted in mlm_dropped_targets.  0: the head runs on every token
+    max_predictions_per_seq: int = 0
 
 
 class BertEmbeddings(nn.Module):
@@ -114,6 +119,8 @@ class BertForPreTraining(nn.Module):
         self.mlm_norm = nn.LayerNorm(c.hidden_size, eps=c.layer_norm_eps)
         self.mlm_bias = nn.Parameter(torch.zeros(c.vocab_size))
         self.nsp = nn.Linear(c.hidden_size, 2)
+        # labelled tokens that found no slot of the max_predictions_per_seq head, summed over every forward
+        self.register_buffer("mlm_dropped_targets", torch.zeros((), dtype=torch.int64), persistent=False)
         self.apply(self._init)
 
     @staticmethod
@@ -130,7 +137,11 @@ class BertForPreTraining(nn.Module):
         None.  Token t takes position t - cu[n], NSP pools the first token of each sequence (``nsp_labels`` [N], -100
         for empty slots), tokens outside every sequence take no MLM loss, and attention stays inside each sequence.
         ``max_seqlen`` (default min(S, max_position)) bounds every length.  Nothing here reads cu_seqlens on the host,
-        so a step with fixed shapes captures into one CUDA graph."""
+        so a step with fixed shapes captures into one CUDA graph.
+
+        With ``config.max_predictions_per_seq`` = k > 0 and ``mlm_labels``, the MLM head runs on the first B k
+        labelled tokens in stream order only (in packed mode k counts per row of the B x S stream); the labelled
+        tokens past them take no loss and are added to ``mlm_dropped_targets``."""
         if type_ids is None:
             type_ids = torch.zeros_like(ids)
         pos = first = None
@@ -150,6 +161,9 @@ class BertForPreTraining(nn.Module):
         for layer in self.layers:
             x = layer(x, mask, cu_seqlens, max_seqlen)
         pooled = torch.tanh(self.pooler(x[:, 0] if first is None else x.reshape(-1, x.shape[-1])[first]))
+        if mlm_labels is not None and self.config.max_predictions_per_seq > 0:
+            x, mlm_labels, dropped = gather_labelled(x, mlm_labels, x.shape[0] * self.config.max_predictions_per_seq)
+            self.mlm_dropped_targets.add_(dropped)
         h = self.mlm_norm(F.gelu(self.mlm_dense(x)))
         logits = F.linear(h, self.embeddings.word.weight, self.mlm_bias)   # tied decoder
         nsp_logits = self.nsp(pooled)

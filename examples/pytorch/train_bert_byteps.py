@@ -32,6 +32,9 @@ p.add_argument("--optimizer", choices=("adamw", "lamb"), default="adamw",
                help="lamb: weights with decay and the trust ratio; biases and LayerNorm weights without either")
 p.add_argument("--max-grad-norm", type=float, default=None,
                help="clip the averaged gradients by their global 2-norm before every update (BERT recipes use 1.0)")
+p.add_argument("--max-predictions-per-seq", type=int, default=None,
+               help="label 15 %% of the positions and run the masked-LM head on at most this many per sequence "
+                    "(BERT recipes use 20 at 128 tokens, 80 at 512)")
 args = p.parse_args()
 bps.init()
 cuda = torch.cuda.is_available() and not args.no_cuda
@@ -39,7 +42,8 @@ if cuda:
     torch.cuda.set_device(bps.local_rank())
 dev = torch.device("cuda", bps.local_rank()) if cuda else torch.device("cpu")
 model = get_model(args.model, fused_norm=args.fused_norm, fused_loss=args.fused_loss,
-                  fp8_linear=args.fp8_linear, fused_attention=args.fused_attention).to(dev)
+                  fp8_linear=args.fp8_linear, fused_attention=args.fused_attention,
+                  max_predictions_per_seq=args.max_predictions_per_seq or 0).to(dev)
 if cuda:
     model = model.to(torch.bfloat16)
 if args.optimizer == "lamb":
@@ -55,6 +59,8 @@ opt = bps.DistributedOptimizer(inner, named_parameters=model.named_parameters(),
 bps.broadcast_parameters(model.state_dict(), root_rank=0)
 ids = torch.randint(0, 30522, (args.batch_size, args.seq_len), device=dev)
 labels = torch.randint(0, 30522, (args.batch_size, args.seq_len), device=dev)
+if args.max_predictions_per_seq:
+    labels[torch.rand(labels.shape, device=dev) >= 0.15] = -100
 
 
 def sync():
