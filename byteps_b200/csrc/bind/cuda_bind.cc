@@ -253,4 +253,5 @@ PYBIND11_MODULE(_cuda, m) {
   bind_cuda_clip(m);
   bind_cuda_attn(m);
   bind_cuda_mlm(m);
+  bind_cuda_stem(m);
 }

@@ -15,3 +15,4 @@ void bind_cuda_lars(pybind11::module_& m);
 void bind_cuda_clip(pybind11::module_& m);
 void bind_cuda_attn(pybind11::module_& m);
 void bind_cuda_mlm(pybind11::module_& m);
+void bind_cuda_stem(pybind11::module_& m);

@@ -1,6 +1,7 @@
 // Tile code shared by the padded (attn.cu) and packed variable-length (attn_varlen.cu) attention kernels: cp.async
 // tile loads into XOR-swizzled shared memory, ldmatrix + mma.sync.m16n8k16 products with fp32 accumulators, the
-// dropout keep bits of a tile, and the host-side launch helpers.  Included only by those two translation units.
+// dropout keep bits of a tile, and the host-side launch helpers.  Included by those two translation units and by
+// the stem convolution (stem_conv.cu), which uses the tile loads and the ldmatrix / mma wrappers.
 #pragma once
 #include <type_traits>
 

@@ -11,6 +11,7 @@ import torch
 import torch.nn as nn
 
 from ..ops.bn_act import BatchNormAct2d
+from ..ops.stem_conv import StemConv2d
 
 
 def _conv3x3(i, o, stride=1):
@@ -64,7 +65,7 @@ class ResNet(nn.Module):
     def __init__(self, block, layers, num_classes=1000, zero_init_residual=False):
         super().__init__()
         self.inplanes = 64
-        self.conv1 = nn.Conv2d(3, 64, 7, 2, 3, bias=False)
+        self.conv1 = StemConv2d(3, 64, 7, 2, 3, bias=False)
         self.bn1 = BatchNormAct2d(64, act="relu")
         self.maxpool = nn.MaxPool2d(3, 2, 1)
         self.layer1 = self._make_layer(block, 64, layers[0])
