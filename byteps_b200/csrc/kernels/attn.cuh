@@ -35,6 +35,15 @@
 // Dropout keeps element (head h, query token t, key token u of sequence n) when word i % 4 of the Philox block with
 // counter (i / 4, offset) is below `keep`, where i = (h T + t) * 512 + (u - cu[n]): the padded numbering with the
 // batch row replaced by the token and the key stride fixed at the longest supported sequence.
+//
+// Causal mask (causal = true, attn_causal.cu): query q attends to key k only when k <= q, in the padded form with
+// q and k the positions in the batch row and in the packed form the positions within the sequence (t - cu[n] and
+// u - cu[n]).  A key-padding mask still applies on top: a query row whose allowed keys are all masked gets a zero
+// context, lse = +inf and zero gradients, as above.  The dropout numbering is the one above, so an element a causal
+// call keeps is one the bidirectional call with the same (seed, offset) keeps.  Forward and the dQ launch of query
+// tile x visit key tiles 0 .. x only and the dK / dV launch of key tile y query tiles y .. last, masking the diagonal
+// tile element by element; everything else above holds unchanged, and it is still one launch forward and two
+// backward.
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -49,19 +58,19 @@ enum AttnMaskKind { ATTN_MASK_F32 = 0, ATTN_MASK_BF16 = 1, ATTN_MASK_F16 = 2, AT
 
 cudaError_t launch_attn_fwd(const void* qkv, int dtype, int B, int S, int H, int D, const void* mask, int mask_kind,
                             int64_t mask_bstride, const int64_t* seed, uint32_t keep, float scale, void* out,
-                            float* lse, cudaStream_t s);
+                            float* lse, cudaStream_t s, bool causal = false);
 // launch 1 (one CTA per 64-query tile) writes delta and dQ; launch 2 (one CTA per 64-key tile) writes dK and dV
 cudaError_t launch_attn_bwd(const void* qkv, const void* out, const void* dout, const float* lse, int dtype, int B,
                             int S, int H, int D, const void* mask, int mask_kind, int64_t mask_bstride,
                             const int64_t* seed, uint32_t keep, float scale, float* delta, void* dqkv,
-                            cudaStream_t s);
+                            cudaStream_t s, bool causal = false);
 
 cudaError_t launch_attn_varlen_fwd(const void* qkv, int dtype, int T, int N, int H, int D, int max_seqlen,
                                    const int* cu_seqlens, const int64_t* seed, uint32_t keep, float scale, void* out,
-                                   float* lse, cudaStream_t s);
+                                   float* lse, cudaStream_t s, bool causal = false);
 cudaError_t launch_attn_varlen_bwd(const void* qkv, const void* out, const void* dout, const float* lse, int dtype,
                                    int T, int N, int H, int D, int max_seqlen, const int* cu_seqlens,
                                    const int64_t* seed, uint32_t keep, float scale, float* delta, void* dqkv,
-                                   cudaStream_t s);
+                                   cudaStream_t s, bool causal = false);
 
 }  // namespace bps

@@ -1,7 +1,7 @@
-// Tile code shared by the padded (attn.cu) and packed variable-length (attn_varlen.cu) attention kernels: cp.async
-// tile loads into XOR-swizzled shared memory, ldmatrix + mma.sync.m16n8k16 products with fp32 accumulators, the
-// dropout keep bits of a tile, and the host-side launch helpers.  Included by those two translation units and by
-// the stem convolution (stem_conv.cu), which uses the tile loads and the ldmatrix / mma wrappers.
+// Tile code shared by the padded (attn_kernels.cuh) and packed variable-length (attn_varlen_kernels.cuh) attention
+// kernels: cp.async tile loads into XOR-swizzled shared memory, ldmatrix + mma.sync.m16n8k16 products with fp32
+// accumulators, the dropout keep bits of a tile, and the host-side launch helpers.  Included by those two headers
+// and by the stem convolution (stem_conv.cu), which uses the tile loads and the ldmatrix / mma wrappers.
 #pragma once
 #include <type_traits>
 
@@ -156,6 +156,16 @@ __device__ __forceinline__ bool row_kept(const uint32_t (*w)[2], int n, int j) {
   return (w[j >> 1][n >> 2] >> ((n & 3) * 8 + 2 * t + (j & 1))) & 1u;
 }
 
+// the query tile of a CTA that walks one query tile over the key tiles: under the causal mask the last tile first,
+// so the CTAs with the most key tiles start first
+template <bool CAUSAL>
+__device__ __forceinline__ int query_tile() {
+  return CAUSAL ? (int)(gridDim.x - 1 - blockIdx.x) : (int)blockIdx.x;
+}
+
+// whether the score of tile row r and tile column c lies above the diagonal of a diagonal tile (causal mask)
+__device__ __forceinline__ bool above_diagonal(int r, int c) { return c > r; }
+
 template <bool BF>
 __device__ __forceinline__ float dot8(const uint16_t* x, const uint16_t* y) {
   using U = typename std::conditional<BF, TagBF16, TagF16>::type;
@@ -188,18 +198,18 @@ cudaError_t launch(F kernel, int smem, bool* raised, dim3 grid, const A& a, cuda
   return cudaGetLastError();
 }
 
-#define ATTN_KERNEL(NAME, BF, DROP, SMEM)              \
-  {                                                    \
-    static bool raised[kMaxDevices];                   \
-    return launch(NAME<BF, DROP>, SMEM, raised, grid, a, s); \
+#define ATTN_KERNEL(NAME, BF, DROP, CAUSAL, SMEM)                    \
+  {                                                                   \
+    static bool raised[kMaxDevices];                                  \
+    return launch(NAME<BF, DROP, CAUSAL>, SMEM, raised, grid, a, s);  \
   }
-#define ATTN_DISPATCH(NAME, SMEM)                                   \
+#define ATTN_DISPATCH(NAME, SMEM, CAUSAL)                           \
   if (bf) {                                                         \
-    if (drop) ATTN_KERNEL(NAME, true, true, SMEM)                   \
-    else ATTN_KERNEL(NAME, true, false, SMEM)                       \
+    if (drop) ATTN_KERNEL(NAME, true, true, CAUSAL, SMEM)           \
+    else ATTN_KERNEL(NAME, true, false, CAUSAL, SMEM)               \
   } else {                                                          \
-    if (drop) ATTN_KERNEL(NAME, false, true, SMEM)                  \
-    else ATTN_KERNEL(NAME, false, false, SMEM)                      \
+    if (drop) ATTN_KERNEL(NAME, false, true, CAUSAL, SMEM)          \
+    else ATTN_KERNEL(NAME, false, false, CAUSAL, SMEM)              \
   }
 
 bool aligned16(const void* p) { return ((uintptr_t)p & 15u) == 0; }

@@ -27,6 +27,13 @@ max_seqlen <= 512, three kernels of kernels/attn_varlen.cu run; a sequence longe
 its context and gradient rows.  Every other input runs SDPA over the whole stream with a block-diagonal additive mask
 built on the device.  Dropout element (h, t, u) of sequence n, for query token t and key token u, has index
 i = (h T + t) 512 + (u - cu[n]) in the same Philox scheme.
+
+Causal attention: with ``causal=True`` query q attends to key k only when k <= q (in the packed form, positions within
+the sequence), on top of any key-padding mask.  The kernels then visit only the key tiles on or below the diagonal
+(kernels/attn_causal.cu), about half the work at S = 512; the fast-path conditions and the dropout numbering are the
+ones above, so a kept element is one the bidirectional call with the same seed keeps.  Every other input runs the
+stock expression with the causal mask: SDPA with ``is_causal=True`` without a mask, an explicit combined mask with one
+(SDPA takes only one of the two), and for packed streams the block-diagonal mask intersected with t >= u.
 """
 from __future__ import annotations
 
@@ -46,18 +53,31 @@ _HEAD_DIM = 64
 _MAX_SEQ = 512
 
 
-def _stock(qkv, num_heads, mask, p):
-    """The expression models/bert.py runs without fused attention."""
+def _causal_mask(mask, s, device):
+    """``mask`` combined with the causal mask k <= q, as one bool or additive mask broadcast to [..., S, S]"""
+    allowed = torch.ones(s, s, dtype=torch.bool, device=device).tril_()
+    if mask.dtype == torch.bool:
+        return mask & allowed
+    return torch.where(allowed, mask, torch.full((), float("-inf"), dtype=mask.dtype, device=device))
+
+
+def _stock(qkv, num_heads, mask, p, causal=False):
+    """The expression models/bert.py runs without fused attention, with the causal mask when ``causal``."""
     b, s, e3 = qkv.shape
     e = e3 // 3
     q, k, v = qkv.view(b, s, 3, num_heads, e // num_heads).permute(2, 0, 3, 1, 4)
-    a = F.scaled_dot_product_attention(q, k, v, attn_mask=mask, dropout_p=p)
+    if causal and mask is not None:
+        a = F.scaled_dot_product_attention(q, k, v, attn_mask=_causal_mask(mask, s, qkv.device), dropout_p=p)
+    elif causal:
+        a = F.scaled_dot_product_attention(q, k, v, dropout_p=p, is_causal=True)
+    else:
+        a = F.scaled_dot_product_attention(q, k, v, attn_mask=mask, dropout_p=p)
     return a.transpose(1, 2).reshape(b, s, e)
 
 
 class _SelfAttentionFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, qkv, mask, num_heads, p):
+    def forward(ctx, qkv, mask, num_heads, p, causal):
         cu = _native.cuda()
         qkv = _aligned(qkv)
         b, s, e3 = qkv.shape
@@ -73,7 +93,9 @@ class _SelfAttentionFn(torch.autograd.Function):
                     _keep_threshold(p) if p > 0.0 else 0, 1.0 / (1.0 - p))
         code, _, _, _, _, _, _, keep, scale = ctx.args
         cu.attn_fwd(qkv.data_ptr(), code, b, s, num_heads, _HEAD_DIM, _ptr(mask), kind, bstride, _ptr(seed), keep,
-                    scale, out.data_ptr(), lse.data_ptr(), torch.cuda.current_stream(qkv.device).cuda_stream)
+                    scale, out.data_ptr(), lse.data_ptr(), torch.cuda.current_stream(qkv.device).cuda_stream,
+                    causal=causal)
+        ctx.causal = causal
         ctx.save_for_backward(qkv, out, lse, mask, seed)
         return out
 
@@ -87,8 +109,8 @@ class _SelfAttentionFn(torch.autograd.Function):
         dqkv = torch.empty_like(qkv)
         cu.attn_bwd(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr(), code, b, s, h, d, _ptr(mask),
                     kind, bstride, _ptr(seed), keep, scale, delta.data_ptr(), dqkv.data_ptr(),
-                    torch.cuda.current_stream(qkv.device).cuda_stream)
-        return dqkv, None, None, None
+                    torch.cuda.current_stream(qkv.device).cuda_stream, causal=ctx.causal)
+        return dqkv, None, None, None, None
 
 
 def _key_padding(mask, b, s, device):
@@ -109,8 +131,9 @@ def _packed_tokens(cu_seqlens, t):
     return seq.clamp(0, n - 1), inside
 
 
-def _stock_varlen(qkv, num_heads, cu_seqlens, max_seqlen, p):
-    """SDPA over the whole stream with a block-diagonal additive mask, the expression the packed kernels compute.
+def _stock_varlen(qkv, num_heads, cu_seqlens, max_seqlen, p, causal=False):
+    """SDPA over the whole stream with a block-diagonal additive mask, the expression the packed kernels compute; with
+    ``causal`` the mask also requires key token <= query token.
 
     A token outside every sequence attends to itself only, so no row of the mask is all -inf (which SDPA turns into
     NaN on some backends), and its context is zeroed.  A sequence longer than max_seqlen gets NaN rows, as the
@@ -121,6 +144,8 @@ def _stock_varlen(qkv, num_heads, cu_seqlens, max_seqlen, p):
     t = torch.arange(t_all, device=qkv.device)
     seq, inside = _packed_tokens(cu_seqlens, t)
     allowed = (seq[:, None] == seq[None, :]) & inside[:, None] & inside[None, :]
+    if causal:
+        allowed &= t[:, None] >= t[None, :]
     allowed |= torch.eye(t_all, dtype=torch.bool, device=qkv.device)
     mask = torch.zeros(t_all, t_all, dtype=qkv.dtype, device=qkv.device).masked_fill_(~allowed, float("-inf"))
     out = _stock(x.unsqueeze(0), num_heads, mask, p)[0]
@@ -132,7 +157,7 @@ def _stock_varlen(qkv, num_heads, cu_seqlens, max_seqlen, p):
 
 class _VarlenAttentionFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, qkv, cu_seqlens, num_heads, max_seqlen, p):
+    def forward(ctx, qkv, cu_seqlens, num_heads, max_seqlen, p, causal):
         cu = _native.cuda()
         qkv = _aligned(qkv)
         e3 = qkv.shape[-1]
@@ -147,7 +172,8 @@ class _VarlenAttentionFn(torch.autograd.Function):
         code, _, n, _, _, _, keep, scale = ctx.args
         cu.attn_varlen_fwd(qkv.data_ptr(), code, t, n, num_heads, _HEAD_DIM, max_seqlen, cu_seqlens.data_ptr(),
                            _ptr(seed), keep, scale, out.data_ptr(), lse.data_ptr(),
-                           torch.cuda.current_stream(qkv.device).cuda_stream)
+                           torch.cuda.current_stream(qkv.device).cuda_stream, causal=causal)
+        ctx.causal = causal
         ctx.save_for_backward(qkv, out, lse, cu_seqlens, seed)
         return out
 
@@ -161,11 +187,11 @@ class _VarlenAttentionFn(torch.autograd.Function):
         dqkv = torch.empty_like(qkv)
         cu.attn_varlen_bwd(qkv.data_ptr(), out.data_ptr(), dout.data_ptr(), lse.data_ptr(), code, t, n, h, d,
                            max_seqlen, cu_seqlens.data_ptr(), _ptr(seed), keep, scale, delta.data_ptr(),
-                           dqkv.data_ptr(), torch.cuda.current_stream(qkv.device).cuda_stream)
-        return dqkv, None, None, None, None
+                           dqkv.data_ptr(), torch.cuda.current_stream(qkv.device).cuda_stream, causal=ctx.causal)
+        return dqkv, None, None, None, None, None
 
 
-def _varlen(qkv, num_heads, mask, p, cu_seqlens, max_seqlen):
+def _varlen(qkv, num_heads, mask, p, cu_seqlens, max_seqlen, causal):
     if mask is not None:
         raise ValueError("mask and cu_seqlens cannot be used together")
     if (not isinstance(cu_seqlens, torch.Tensor) or cu_seqlens.dim() != 1 or cu_seqlens.dtype != torch.int32
@@ -183,24 +209,25 @@ def _varlen(qkv, num_heads, mask, p, cu_seqlens, max_seqlen):
     fusable = (qkv.is_cuda and qkv.dtype in _CODES and e3 // (3 * num_heads) == _HEAD_DIM and t >= 1
                and max_seqlen <= _MAX_SEQ and n <= 65535 and num_heads <= 65535 and qkv.is_contiguous() and p < 1.0)
     if not fusable:
-        return _stock_varlen(qkv, num_heads, cu_seqlens, max_seqlen, p)
-    return _VarlenAttentionFn.apply(qkv, cu_seqlens.contiguous(), num_heads, max_seqlen, p)
+        return _stock_varlen(qkv, num_heads, cu_seqlens, max_seqlen, p, causal)
+    return _VarlenAttentionFn.apply(qkv, cu_seqlens.contiguous(), num_heads, max_seqlen, p, causal)
 
 
 def self_attention(qkv: torch.Tensor, num_heads: int, mask: Optional[torch.Tensor] = None, p: float = 0.0,
                    training: bool = True, *, cu_seqlens: Optional[torch.Tensor] = None,
-                   max_seqlen: Optional[int] = None) -> torch.Tensor:
+                   max_seqlen: Optional[int] = None, causal: bool = False) -> torch.Tensor:
     """The [B, S, E] context of multi-head self-attention over ``qkv`` = [B, S, 3E] (Q, K, V of ``num_heads`` heads
     each), with the additive or boolean ``mask`` of ``F.scaled_dot_product_attention`` and dropout ``p`` on the
     attention probabilities when ``training``.
 
     With ``cu_seqlens`` the rows of ``qkv`` are one packed stream of sequences (see the module docstring), ``mask``
-    must be None, and the result has ``qkv``'s shape with E columns."""
+    must be None, and the result has ``qkv``'s shape with E columns.  With ``causal`` query q attends to key k only
+    when k <= q (positions within the sequence for a packed stream), on top of ``mask``."""
     if not 0.0 <= p <= 1.0:
         raise ValueError("dropout probability has to be between 0 and 1, but got %r" % (p,))
     p = float(p) if training else 0.0
     if cu_seqlens is not None:
-        return _varlen(qkv, num_heads, mask, p, cu_seqlens, max_seqlen)
+        return _varlen(qkv, num_heads, mask, p, cu_seqlens, max_seqlen, bool(causal))
     if max_seqlen is not None:
         raise ValueError("max_seqlen is only taken together with cu_seqlens")
     if qkv.dim() != 3 or qkv.shape[-1] % (3 * num_heads) != 0:
@@ -211,5 +238,5 @@ def self_attention(qkv: torch.Tensor, num_heads: int, mask: Optional[torch.Tenso
     if fusable:
         kp = _key_padding(mask, b, s, qkv.device)
         if mask is None or kp is not None:
-            return _SelfAttentionFn.apply(qkv, kp, num_heads, p)
-    return _stock(qkv, num_heads, mask, p)
+            return _SelfAttentionFn.apply(qkv, kp, num_heads, p, bool(causal))
+    return _stock(qkv, num_heads, mask, p, bool(causal))
