@@ -8,12 +8,19 @@ kernel names of one profiled fwd+bwd.  As in attn_bench.py, each timed call runs
 and dout that they span more than --rotate-mb together, so no call finds its inputs in the 50 MB L2; --iters calls
 are captured in one CUDA graph and its replays are timed with CUDA events.
 
-Whole step: gpt2_small (124 M) in bf16 at 16 x 512, fused AdamW through DistributedOptimizer(fused_update=True),
-the whole step in one CUDA graph: stock (SDPA, F.cross_entropy), fused_attention + fused_loss, and those with
-fp8_linear.  The arms are separate models with the same initial weights, timed alternately over --rounds rounds of
---steps replays; medians and spreads.  The GPU name, power limit and SM clock are read in the same run.
+Per junction of the pre-LN residual stream, bf16 8192 x 768 with bf16 gamma / beta and p = 0.1: fwd and fwd+bwd
+(torch.autograd.grad to y, residual, gamma and beta, with gradients arriving at both the LayerNorm's output and the
+sum z) of DropoutAddLayerNorm with return_sum=True against the stock z = residual + F.dropout(y), F.layer_norm(z);
+rotated copies and graphed replays as above.
 
-    python benchmarks/gpt_bench.py [--iters 20] [--rotate-mb 200] [--steps 20] [--rounds 5] [--no-step] [--json f]
+Whole step: gpt2_small (124 M) in bf16 at 16 x 512, fused AdamW through DistributedOptimizer(fused_update=True),
+the whole step in one CUDA graph: stock (SDPA, F.cross_entropy), fused_attention + fused_loss, that with fused_norm,
+and those two with fp8_linear.  The arms are separate models with the same initial weights, timed alternately over
+--rounds rounds of --steps replays; medians and spreads.  The GPU name, power limit and SM clock are read in the
+same run.
+
+    python benchmarks/gpt_bench.py [--iters 20] [--rotate-mb 200] [--steps 20] [--rounds 5] [--no-step]
+                                   [--no-call] [--no-junction] [--json f]
 """
 import argparse
 import json
@@ -31,31 +38,33 @@ D = 64
 SHAPES = [(16, 512, 12), (8, 512, 16), (64, 128, 12)]
 
 
+def graphed_us(args, torch, fn, k):
+    """us per call of fn(i % k), --iters calls captured in one graph, timed over --reps replays"""
+    for i in range(k):
+        fn(i)
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        for i in range(args.iters):
+            fn(i % k)
+    g.replay()
+    torch.cuda.synchronize()
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    for _ in range(args.reps):
+        g.replay()
+    b.record()
+    torch.cuda.synchronize()
+    us = a.elapsed_time(b) * 1e3 / (args.reps * args.iters)
+    del g
+    return us
+
+
 def per_call(args, torch, rows):
     from byteps_b200.ops.attn import _stock, self_attention
 
     dev = torch.device("cuda", 0)
     dt = torch.bfloat16
-
-    def graphed_us(fn, k):
-        for i in range(k):
-            fn(i)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            for i in range(args.iters):
-                fn(i % k)
-        g.replay()
-        torch.cuda.synchronize()
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        for _ in range(args.reps):
-            g.replay()
-        b.record()
-        torch.cuda.synchronize()
-        us = a.elapsed_time(b) * 1e3 / (args.reps * args.iters)
-        del g
-        return us
 
     print("%-12s %-4s %-14s %-8s %9s" % ("B x S x H", "p", "path", "pass", "us"))
     for (b, s, h) in SHAPES:
@@ -78,7 +87,7 @@ def per_call(args, torch, rows):
                     x, dout = T[i]
                     torch.autograd.grad(f(x), [x], dout)
 
-                us_f, us_fb = graphed_us(fwd, k), graphed_us(both, k)
+                us_f, us_fb = graphed_us(args, torch, fwd, k), graphed_us(args, torch, both, k)
                 res[path] = (us_f, us_fb)
                 backend = sdpa_backend(torch, both) if path == "causal_sdpa" else "byteps_b200 attn kernels"
                 for kind, us in (("fwd", us_f), ("fwd+bwd", us_fb)):
@@ -92,8 +101,51 @@ def per_call(args, torch, rows):
         del T
 
 
+def per_junction(args, torch, rows, m=8192, h=768, p=0.1):
+    import torch.nn.functional as F
+
+    from byteps_b200.ops.ln import dropout_add_layer_norm
+
+    dev = torch.device("cuda", 0)
+    dt = torch.bfloat16
+    per_copy = m * h * 2 * 4
+    k = max(2, int(-(-args.rotate_mb * 1e6 // per_copy)))
+    gen = torch.Generator(device=dev).manual_seed(0)
+    T = [tuple(torch.randn(m, h, device=dev, generator=gen).to(dt) for _ in range(4)) for _ in range(k)]
+    w = torch.ones(h, device=dev, dtype=dt, requires_grad=True)
+    b = torch.zeros(h, device=dev, dtype=dt, requires_grad=True)
+    leaves = [(y.requires_grad_(True), r.requires_grad_(True)) for y, r, _, _ in T]
+
+    def fused(y, r):
+        return dropout_add_layer_norm(y, r, w, b, p, 1e-5, True, return_sum=True)
+
+    def stock(y, r):
+        z = r + F.dropout(y, p, True)
+        return F.layer_norm(z, (h,), w, b, 1e-5), z
+
+    print("%-10s %-6s %-8s %9s" % ("M x H", "path", "pass", "us"))
+    res = {}
+    for path, f in (("fused", fused), ("stock", stock)):
+        def fwd(i, f=f):
+            f(*leaves[i])
+
+        def both(i, f=f):
+            y, r = leaves[i]
+            torch.autograd.grad(f(y, r), [y, r, w, b], [T[i][2], T[i][3]])
+
+        res[path] = (graphed_us(args, torch, fwd, k), graphed_us(args, torch, both, k))
+        for kind, us in zip(("fwd", "fwd+bwd"), res[path]):
+            rows.append(dict(junction=[m, h], p=p, path=path, kind=kind, us=us))
+            print("%-10s %-6s %-8s %9.1f" % ("%dx%d" % (m, h), path, kind, us))
+    print("           stock / fused: fwd %.2fx, fwd+bwd %.2fx" % (res["stock"][0] / res["fused"][0],
+                                                                  res["stock"][1] / res["fused"][1]))
+    del T, leaves
+
+
 ARMS = {"stock": {}, "fused_attn_loss": dict(fused_attention=True, fused_loss=True),
-        "fused_attn_loss_fp8": dict(fused_attention=True, fused_loss=True, fp8_linear=True)}
+        "fused_attn_loss_norm": dict(fused_attention=True, fused_loss=True, fused_norm=True),
+        "fused_attn_loss_fp8": dict(fused_attention=True, fused_loss=True, fp8_linear=True),
+        "fused_attn_loss_fp8_norm": dict(fused_attention=True, fused_loss=True, fp8_linear=True, fused_norm=True)}
 
 
 def whole_step(args, torch, rows, batch, seq):
@@ -159,7 +211,8 @@ def main():
     ap.add_argument("--steps", type=int, default=20, help="timed replays of a whole step per round")
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--no-step", action="store_true", help="per-call table only")
-    ap.add_argument("--no-call", action="store_true", help="whole steps only")
+    ap.add_argument("--no-call", action="store_true", help="no per-call attention table")
+    ap.add_argument("--no-junction", action="store_true", help="no per-junction LayerNorm table")
     ap.add_argument("--json", default=None, help="also write the rows as JSON to this file")
     args = ap.parse_args()
 
@@ -176,6 +229,8 @@ def main():
     rows = []
     if not args.no_call:
         per_call(args, torch, rows)
+    if not args.no_junction:
+        per_junction(args, torch, rows)
     if not args.no_step:
         import byteps_b200.torch as bps
 

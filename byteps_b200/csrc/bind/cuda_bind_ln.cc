@@ -36,13 +36,17 @@ void bind_cuda_ln(py::module_& m) {
      "out = layer_norm(z); keep = (1 - p) * 2^32 and scale = 1 / (1 - p) when mask is given");
   m.def("ln_bwd", [](uintptr_t dout, uintptr_t z, uintptr_t mask, int dtype, int wdtype, size_t M, int H, float scale,
                      uintptr_t mean, uintptr_t rstd, uintptr_t gamma, uintptr_t dres, uintptr_t dy, uintptr_t dgamma,
-                     uintptr_t dbeta, uintptr_t ws, uintptr_t counters, uintptr_t s) {
+                     uintptr_t dbeta, uintptr_t ws, uintptr_t counters, uintptr_t s, uintptr_t dsum) {
     chk(launch_ln_bwd((const void*)dout, (const void*)z, (const uint8_t*)mask, dtype, wdtype, M, H, scale,
                       (const float*)mean, (const float*)rstd, (const void*)gamma, (void*)dres, (void*)dy,
-                      (void*)dgamma, (void*)dbeta, (float*)ws, (uint32_t*)counters, (cudaStream_t)s),
+                      (void*)dgamma, (void*)dbeta, (float*)ws, (uint32_t*)counters, (cudaStream_t)s,
+                      (const void*)dsum),
         "ln_bwd");
   }, py::arg("dout"), py::arg("z"), py::arg("mask"), py::arg("dtype"), py::arg("wdtype"), py::arg("M"), py::arg("H"),
      py::arg("scale"), py::arg("mean"), py::arg("rstd"), py::arg("gamma"), py::arg("dres"), py::arg("dy"),
-     py::arg("dgamma"), py::arg("dbeta"), py::arg("ws"), py::arg("counters"), py::arg("stream"),
-     "dres = dz and dy = dz * mask * scale (each 0 when not wanted), dgamma and dbeta in the parameter dtype");
+     py::arg("dgamma"), py::arg("dbeta"), py::arg("ws"), py::arg("counters"), py::arg("stream"), py::kw_only(),
+     py::arg("dsum") = 0,
+     "dres = dz and dy = dz * mask * scale (each 0 when not wanted), dgamma and dbeta in the parameter dtype; "
+     "dsum: a second gradient of z in the activation dtype, added to dz (s = round(round(dz) + dsum)) before dres "
+     "and dy are formed from it");
 }

@@ -181,9 +181,12 @@ struct BwdArgs {
   size_t M, rpc;
   int H;
   float scale;
+  const void* dsum;
 };
 
-template <class U, class W, int NU, int TPR>
+// SUM: a second gradient dsum arrives at z (a pre-LN block's residual stream); dz is rounded to the activation dtype
+// and dsum added to it with one more rounding, the sum autograd would have formed, before dres and dy are written.
+template <class U, class W, int NU, int TPR, bool SUM>
 __global__ void __launch_bounds__(kT, kBwdBlocksPerSM) ln_bwd_kernel(BwdArgs a) {
   constexpr int RPB = kT / TPR, NW = TPR > 32 ? TPR / 32 : 1;
   __shared__ float sh[RPB][2][2][NW];
@@ -236,6 +239,14 @@ __global__ void __launch_bounds__(kT, kBwdBlocksPerSM) ln_bwd_kernel(BwdArgs a) 
         float dz[kCh];
 #pragma unroll
         for (int j = 0; j < kCh; ++j) dz[j] = rstd * (g[k][j] - ma - xh[k][j] * mb);
+        if constexpr (SUM) {
+          float ds[kCh];
+          Io<U>::load(a.dsum, gu, ds);
+          Io<U>::round(dz);
+#pragma unroll
+          for (int j = 0; j < kCh; ++j) dz[j] = __fadd_rn(dz[j], ds[j]);   // never contracted into an fma with dz
+          Io<U>::round(dz);
+        }
         if (a.dres != nullptr) Io<U>::store(a.dres, gu, dz);
         if (a.dy != nullptr) {
           const uint32_t bits = a.mask != nullptr ? a.mask[gu] : 0xffu;
@@ -347,7 +358,7 @@ int fwd_wave() {
 template <class U, class W, int NU, int TPR>
 int bwd_wave() {
   static int cache[kMaxDevices];
-  return resident(ln_bwd_kernel<U, W, NU, TPR>, cache) * sm_count();
+  return resident(ln_bwd_kernel<U, W, NU, TPR, false>, cache) * sm_count();
 }
 
 // Contiguous chunks of rows (a multiple of the block's rpb rows per step), at most one per block of a wave.
@@ -411,16 +422,22 @@ cudaError_t launch_ln_fwd(const void* y, const void* residual, int dtype, int wd
 
 cudaError_t launch_ln_bwd(const void* dout, const void* z, const uint8_t* mask, int dtype, int wdtype, size_t M, int H,
                           float scale, const float* mean, const float* rstd, const void* gamma, void* dres, void* dy,
-                          void* dgamma, void* dbeta, float* ws, uint32_t* counters, cudaStream_t s) {
+                          void* dgamma, void* dbeta, float* ws, uint32_t* counters, cudaStream_t s,
+                          const void* dsum) {
   if (bad_shape(M, H) || !aligned16(dout) || !aligned16(z) || !aligned16(gamma) || !aligned16(dres) ||
-      !aligned16(dy) || dout == nullptr || z == nullptr || gamma == nullptr || mean == nullptr || rstd == nullptr ||
-      dgamma == nullptr || dbeta == nullptr || ws == nullptr || counters == nullptr)
+      !aligned16(dy) || !aligned16(dsum) || dout == nullptr || z == nullptr || gamma == nullptr || mean == nullptr ||
+      rstd == nullptr || dgamma == nullptr || dbeta == nullptr || ws == nullptr || counters == nullptr)
     return cudaErrorInvalidValue;
-  BwdArgs a{dout, z, gamma, mask, mean, rstd, dres, dy, dgamma, dbeta, ws, counters, M, 0, H, scale};
+  BwdArgs a{dout, z, gamma, mask, mean, rstd, dres, dy, dgamma, dbeta, ws, counters, M, 0, H, scale, dsum};
+  // Both variants take the grid of the one without dsum, so dgamma and dbeta are summed in the same order (and the
+  // workspace sized for it suffices); no block waits for another, so the grid need not be resident at once.
   LN_DISPATCH(dtype, wdtype, H, ({
     int grid;
     chunks(M, kT / TPR, bwd_wave<U, W, NU, TPR>(), &a.rpc, &grid);
-    ln_bwd_kernel<U, W, NU, TPR><<<grid, kT, 0, s>>>(a);
+    if (dsum != nullptr)
+      ln_bwd_kernel<U, W, NU, TPR, true><<<grid, kT, 0, s>>>(a);
+    else
+      ln_bwd_kernel<U, W, NU, TPR, false><<<grid, kT, 0, s>>>(a);
   }));
   return cudaGetLastError();
 }

@@ -10,7 +10,10 @@
 //         nullptr.
 //   bwd   g = dout * gamma, xhat = (z - mean) * rstd, dz = rstd * (g - mean_H(g) - xhat * mean_H(g * xhat));
 //         writes dres = dz and dy = dz * mask * scale, each when its pointer is given (mask nullptr: dy = dz * scale),
-//         and dgamma = sum dout * xhat, dbeta = sum dout over the rows.
+//         and dgamma = sum dout * xhat, dbeta = sum dout over the rows.  With dsum (the gradient reaching z from
+//         everything but this LayerNorm, as in a pre-LN block where z is also the residual stream; activation dtype,
+//         same layout as dout) dz is first replaced by s = round(round(dz) + dsum), the sum autograd would form, so
+//         dres = s and dy = round(s * scale) on kept elements, 0 on dropped ones.  dsum == nullptr: as before.
 //
 // Dropout keeps element i = row * H + col when word i % 4 of Philox4x32-10 (key = seed, counter = (i / 4, offset),
 // 64 bits each, low word first) is below `keep` (= (1 - p) * 2^32), and scales kept values by `scale` (1 / (1 - p)).
@@ -40,6 +43,7 @@ cudaError_t launch_ln_fwd(const void* y, const void* residual, int dtype, int wd
                           void* z, void* out, float* mean, float* rstd, uint8_t* mask, cudaStream_t s);
 cudaError_t launch_ln_bwd(const void* dout, const void* z, const uint8_t* mask, int dtype, int wdtype, size_t M, int H,
                           float scale, const float* mean, const float* rstd, const void* gamma, void* dres, void* dy,
-                          void* dgamma, void* dbeta, float* ws, uint32_t* counters, cudaStream_t s);
+                          void* dgamma, void* dbeta, float* ws, uint32_t* counters, cudaStream_t s,
+                          const void* dsum = nullptr);
 
 }  // namespace bps

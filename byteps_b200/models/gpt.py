@@ -9,6 +9,7 @@ import torch.nn.functional as F
 
 from ..ops.attn import _packed_tokens, _stock, _stock_varlen, self_attention
 from ..ops.fp8 import Fp8Linear, fp8_gelu_mlp
+from ..ops.ln import DropoutAddLayerNorm
 from ..ops.xent import softmax_cross_entropy
 
 
@@ -33,39 +34,60 @@ class GptConfig:
     # qkv, proj, fc1 and fc2 of every block as ops.fp8.Fp8Linear with the GELU inside the FP8 casts
     # (ops.fp8.fp8_gelu_mlp); same parameters and state_dict as nn.Linear.  The LM head stays in the model's dtype
     fp8_linear: bool = False
+    # every LayerNorm (ln1, ln2, ln_f) as ops.ln.DropoutAddLayerNorm, run with the dropout and residual add in front
+    # of it and returning their sum as the residual stream: one fused kernel per direction on CUDA at each of the
+    # 2 L + 1 junctions (same parameters and state_dict; other inputs run the stock composition)
+    fused_norm: bool = False
 
 
 def _block_linear(c: GptConfig, i: int, o: int) -> nn.Linear:
     return Fp8Linear(i, o) if c.fp8_linear else nn.Linear(i, o)
 
 
+def _norm(c: GptConfig) -> nn.LayerNorm:
+    if c.fused_norm:
+        return DropoutAddLayerNorm(c.hidden_size, eps=c.layer_norm_eps, p=c.dropout)
+    return nn.LayerNorm(c.hidden_size, eps=c.layer_norm_eps)
+
+
 class GptBlock(nn.Module):
-    """x + drop(proj(attn(ln1(x)))), then x + drop(mlp(ln2(x)))"""
+    """x + drop(proj(attn(ln1(x)))), then x + drop(mlp(ln2(x))).  With fused_norm the model runs the block
+    through fused_forward instead, where each LayerNorm also forms the residual sum in front of it."""
 
     def __init__(self, c: GptConfig):
         super().__init__()
         self.h = c.num_heads
-        self.ln1 = nn.LayerNorm(c.hidden_size, eps=c.layer_norm_eps)
+        self.ln1 = _norm(c)
         self.qkv = _block_linear(c, c.hidden_size, 3 * c.hidden_size)
         self.proj = _block_linear(c, c.hidden_size, c.hidden_size)
-        self.ln2 = nn.LayerNorm(c.hidden_size, eps=c.layer_norm_eps)
+        self.ln2 = _norm(c)
         self.fc1 = _block_linear(c, c.hidden_size, c.intermediate_size)
         self.fc2 = _block_linear(c, c.intermediate_size, c.hidden_size)
         self.p = c.dropout
         self.fused_attention = c.fused_attention
+        self.fused_norm = c.fused_norm
 
     def forward(self, x, cu_seqlens=None, max_seqlen=None):
-        qkv = self.qkv(self.ln1(x))
-        p = self.p if self.training else 0.0
-        if self.fused_attention:
-            a = self_attention(qkv, self.h, None, self.p, self.training, cu_seqlens=cu_seqlens,
-                               max_seqlen=max_seqlen, causal=True)
-        elif cu_seqlens is not None:
-            a = _stock_varlen(qkv, self.h, cu_seqlens, max_seqlen, p, causal=True)
-        else:
-            a = _stock(qkv, self.h, None, p, causal=True)
+        if self.fused_norm:
+            raise RuntimeError("a fused_norm block runs through fused_forward")
+        a = self.attn(self.qkv(self.ln1(x)), cu_seqlens, max_seqlen)
         x = x + F.dropout(self.proj(a), self.p, self.training)
         return x + F.dropout(self.mlp(self.ln2(x)), self.p, self.training)
+
+    def fused_forward(self, x, a, next_ln, cu_seqlens=None, max_seqlen=None):
+        """(x, a = ln1(x)) -> (next_ln(x'), x') for the block's output x', where next_ln is the next block's ln1
+        or the final ln_f: each LayerNorm takes the dropout and residual add in front of it and returns the sum."""
+        b, h = self.ln2(self.proj(self.attn(self.qkv(a), cu_seqlens, max_seqlen)), residual=x, return_sum=True)
+        return next_ln(self.mlp(b), residual=h, return_sum=True)
+
+    def attn(self, qkv, cu_seqlens, max_seqlen):
+        if self.fused_attention:
+            return self_attention(qkv, self.h, None, self.p, self.training, cu_seqlens=cu_seqlens,
+                                  max_seqlen=max_seqlen, causal=True)
+        p = self.p if self.training else 0.0
+        if cu_seqlens is not None:
+            return _stock_varlen(qkv, self.h, cu_seqlens, max_seqlen, p, causal=True)
+        return _stock(qkv, self.h, None, p, causal=True)
 
     def mlp(self, x):
         if isinstance(self.fc1, Fp8Linear):
@@ -80,7 +102,7 @@ class GptLMHeadModel(nn.Module):
         self.wte = nn.Embedding(c.vocab_size, c.hidden_size)
         self.wpe = nn.Embedding(c.max_position, c.hidden_size)
         self.blocks = nn.ModuleList([GptBlock(c) for _ in range(c.num_layers)])
-        self.ln_f = nn.LayerNorm(c.hidden_size, eps=c.layer_norm_eps)
+        self.ln_f = _norm(c)
         self.apply(self._init)
         # GPT-2 scales the projections that feed the residual stream by 1 / sqrt(2 L)
         for blk in self.blocks:
@@ -113,10 +135,19 @@ class GptLMHeadModel(nn.Module):
             pos = (t - cu_seqlens[seq]).clamp(0, self.config.max_position - 1).view(b, s)
         else:
             pos = torch.arange(s, device=ids.device).unsqueeze(0)
-        x = F.dropout(self.wte(ids) + self.wpe(pos), self.config.dropout, self.training)
-        for blk in self.blocks:
-            x = blk(x, cu_seqlens, max_seqlen)
-        logits = F.linear(self.ln_f(x), self.wte.weight)   # tied LM head
+        e = self.wte(ids) + self.wpe(pos)
+        if self.config.fused_norm:
+            # the embedding dropout runs inside the first ln1, each block's last residual add inside the next ln1
+            a, x = self.blocks[0].ln1(e, return_sum=True)
+            for i, blk in enumerate(self.blocks):
+                next_ln = self.blocks[i + 1].ln1 if i + 1 < len(self.blocks) else self.ln_f
+                a, x = blk.fused_forward(x, a, next_ln, cu_seqlens, max_seqlen)
+        else:
+            x = F.dropout(e, self.config.dropout, self.training)
+            for blk in self.blocks:
+                x = blk(x, cu_seqlens, max_seqlen)
+            a = self.ln_f(x)
+        logits = F.linear(a, self.wte.weight)   # tied LM head
         if labels is None:
             return logits
         # shift the labels rather than the logits, so the [T, V] logits stay one contiguous tensor

@@ -11,6 +11,10 @@ each way.  Every other input takes the stock ``F.dropout`` / add / ``F.layer_nor
 same function.  A tensor whose data does not start on a 16-byte boundary (a view at an odd element offset) is copied
 to one that does before the kernels read it.
 
+``return_sum=True`` also returns z, differentiable, for a pre-LN block, where z is both the LayerNorm's input and
+the residual stream: the backward kernel then adds z's own incoming gradient to the LayerNorm's before it forms
+d(residual) and dy, in place of autograd's separate add.
+
 Dropout bits come from Philox4x32-10 keyed by a (seed, offset) pair drawn on the device from torch's CUDA generator
 on every call, so ``torch.manual_seed`` reproduces them and each replay of a captured CUDA graph draws new ones.
 """
@@ -46,7 +50,7 @@ def _keep_threshold(p: float) -> int:
 
 class _DropoutAddLayerNormFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, y, residual, weight, bias, p, eps, grad):
+    def forward(ctx, y, residual, weight, bias, p, eps, grad, return_sum):
         cu = _native.cuda()
         y, residual, weight, bias = _aligned(y), _aligned(residual), _aligned(weight), _aligned(bias)
         h = y.shape[-1]
@@ -62,26 +66,39 @@ class _DropoutAddLayerNormFn(torch.autograd.Function):
             mask = torch.empty(y.shape[:-1] + (h // _UNIT,), dtype=torch.uint8, device=y.device)
             # (seed, offset) from torch's generator: graph-safe, so every replay of a captured step gets new bits
             seed = torch.randint(0, 2 ** 62, (2,), dtype=torch.int64, device=y.device)
-        # z is y when nothing is added or dropped, and only a backward reads it
-        z = torch.empty_like(y) if grad and (drop or residual is not None) else None
+        # z is y when nothing is added or dropped; otherwise it is written when a backward or the caller reads it
+        z = torch.empty_like(y) if (grad or return_sum) and (drop or residual is not None) else None
         cu.ln_fwd(y.data_ptr(), _ptr(residual), code, wcode, m, h, float(eps), weight.data_ptr(), bias.data_ptr(),
                   _ptr(seed), _keep_threshold(p) if drop else 0, 1.0 / (1.0 - p), _ptr(z), out.data_ptr(),
                   mean.data_ptr(), rstd.data_ptr(), _ptr(mask), stream)
-        ctx.save_for_backward(y if z is None else z, weight, mean, rstd, mask)
+        if z is None:
+            z = y
+        ctx.save_for_backward(z, weight, mean, rstd, mask)
         ctx.p = p
         ctx.has_residual = residual is not None
+        ctx.return_sum = return_sum
         if mask is not None:
             ctx.mark_non_differentiable(mask)
-        return out, mask
+        if not return_sum:
+            return out, mask
+        # z's own gradient (dsum) may not arrive, as the LayerNorm's may not: None rather than a tensor of zeros
+        ctx.set_materialize_grads(False)
+        return out, z, mask
 
     @staticmethod
-    def backward(ctx, dout, _dmask):
+    def backward(ctx, dout, *rest):
         z, weight, mean, rstd, mask = ctx.saved_tensors
+        dsum = rest[0] if ctx.return_sum else None
+        if dout is None and dsum is None:
+            return (None,) * 8
         cu = _native.cuda()
         h = z.shape[-1]
         m = z.numel() // h
         code, wcode = _CODES[z.dtype], _CODES[weight.dtype]
-        dout = _aligned(dout.to(z.dtype).contiguous())
+        # no gradient through the LayerNorm: its dz is 0 and the kernel passes dsum on
+        dout = torch.zeros_like(z) if dout is None else _aligned(dout.to(z.dtype).contiguous())
+        if dsum is not None:
+            dsum = _aligned(dsum.to(z.dtype).contiguous())
         stream = torch.cuda.current_stream(z.device).cuda_stream
         dweight, dbias = torch.empty_like(weight), torch.empty_like(weight)
         dres = torch.empty_like(z) if ctx.has_residual else None
@@ -92,10 +109,10 @@ class _DropoutAddLayerNormFn(torch.autograd.Function):
         ctr = torch.zeros(nctr, dtype=torch.int32, device=z.device)
         cu.ln_bwd(dout.data_ptr(), z.data_ptr(), _ptr(mask), code, wcode, m, h, 1.0 / (1.0 - ctx.p), mean.data_ptr(),
                   rstd.data_ptr(), weight.data_ptr(), _ptr(dres), _ptr(dy), dweight.data_ptr(), dbias.data_ptr(),
-                  ws.data_ptr(), ctr.data_ptr(), stream)
+                  ws.data_ptr(), ctr.data_ptr(), stream, dsum=_ptr(dsum))
         if dy is None:
             dy = dres
-        return dy, dres, dweight, dbias, None, None, None
+        return dy, dres, dweight, dbias, None, None, None, None
 
 
 def _fusable(y, residual, weight, bias, normalized_shape) -> bool:
@@ -112,13 +129,19 @@ def _fusable(y, residual, weight, bias, normalized_shape) -> bool:
 
 def dropout_add_layer_norm(y: torch.Tensor, residual: Optional[torch.Tensor], weight: Optional[torch.Tensor],
                            bias: Optional[torch.Tensor], p: float, eps: float, training: bool,
-                           return_mask: bool = False, normalized_shape: Optional[Sequence[int]] = None):
+                           return_mask: bool = False, normalized_shape: Optional[Sequence[int]] = None,
+                           return_sum: bool = False):
     """``layer_norm(residual + dropout(y, p if training else 0))`` over ``normalized_shape`` (default: the last
     dimension); ``residual`` may be None.
 
-    With ``return_mask`` the result is ``(out, mask)``: the keep mask of the fused kernels, one uint8 per 8
-    elements of a row (bit k = element 8j + k), shaped ``y.shape[:-1] + (H // 8,)``; None when no dropout was
-    applied or the input took the stock composition."""
+    With ``return_sum`` the result is ``(out, z)``, where ``z = residual + dropout(y)`` is the LayerNorm's input
+    and differentiable: in a pre-LN block z is also the residual stream the next junction adds to, and on the fused
+    path its gradient joins the LayerNorm's inside the backward kernel.  z is y itself (a view of it on the fused
+    path) when nothing is added or dropped.
+
+    With ``return_mask`` the mask comes last, ``(out, mask)`` or ``(out, z, mask)``: the keep mask of the fused
+    kernels, one uint8 per 8 elements of a row (bit k = element 8j + k), shaped ``y.shape[:-1] + (H // 8,)``; None
+    when no dropout was applied or the input took the stock composition."""
     if not 0.0 <= p <= 1.0:
         raise ValueError("dropout probability has to be between 0 and 1, but got %r" % (p,))
     p = float(p) if training else 0.0
@@ -126,17 +149,24 @@ def dropout_add_layer_norm(y: torch.Tensor, residual: Optional[torch.Tensor], we
         normalized_shape = tuple(weight.shape) if weight is not None else (y.shape[-1],)
     if p < 1.0 and _fusable(y, residual, weight, bias, normalized_shape):
         grad = torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (y, residual, weight, bias))
-        out, mask = _DropoutAddLayerNormFn.apply(y, residual, weight, bias, p, float(eps), grad)
+        res = _DropoutAddLayerNormFn.apply(y, residual, weight, bias, p, float(eps), grad, return_sum)
+        if return_sum:
+            out, z, mask = res
+        else:
+            out, mask = res
     else:
         z = F.dropout(y, p, training) if p > 0.0 else y
         if residual is not None:
             z = residual + z
         out, mask = F.layer_norm(z, tuple(normalized_shape), weight, bias, eps), None
+    if return_sum:
+        return (out, z, mask) if return_mask else (out, z)
     return (out, mask) if return_mask else out
 
 
 class DropoutAddLayerNorm(nn.LayerNorm):
-    """``nn.LayerNorm`` applied to ``residual + dropout(y, p)``: ``forward(y, residual=None)``.  Dropout is active in
+    """``nn.LayerNorm`` applied to ``residual + dropout(y, p)``: ``forward(y, residual=None, return_sum=False)``,
+    which also returns that sum when ``return_sum`` is set (see ``dropout_add_layer_norm``).  Dropout is active in
     training mode only, as ``nn.Dropout``."""
 
     def __init__(self, normalized_shape, eps=1e-5, elementwise_affine=True, bias=True, p=0.0, device=None,
@@ -149,6 +179,6 @@ class DropoutAddLayerNorm(nn.LayerNorm):
     def extra_repr(self):
         return super().extra_repr() + ", p=%g" % self.p
 
-    def forward(self, y, residual=None):
+    def forward(self, y, residual=None, return_sum=False):
         return dropout_add_layer_norm(y, residual, self.weight, self.bias, self.p, self.eps, self.training,
-                                      normalized_shape=self.normalized_shape)
+                                      normalized_shape=self.normalized_shape, return_sum=return_sum)
